@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (one process per GPU under torchrun)
     python bench.py --impl reference --steps K --warmup W     # the CPU oracle (reference restatement) on the host cores
+    python bench.py --steps K --warmup W --dump-outputs DIR   # + the last timed step's results as DIR/<name>.npy
 
 A "step" is one reverse-diffusion step of the hot path for one batch: set_time -> score-model forward (graph build,
 embeddings, 6 tensor-product conv layers, tr/rot/tor heads) -> pose update, for POSES poses of one synthetic complex
@@ -68,7 +69,7 @@ def peaks():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         return json.load(open(p)), 'measured'
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0}, 'fallback'
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'fallback (H100 SXM data sheet, dense)'
 
 
 class ClockSampler(threading.Thread):
@@ -189,6 +190,9 @@ def run_reference(cli):
         t0 = time.perf_counter()
         step(t_idx)
         costs[t_idx] = time.perf_counter() - t0
+    if cli.dump_outputs:          # the oracle pose after the last timed schedule point [1, atoms, 3]
+        dump_outputs(cli.dump_outputs, {'ligand_pos': step.graph['ligand'].pos.float().reshape(1, -1, 3),
+                                        'step_index': np.array([points[-1]], dtype=np.float64)})
     total = trajectory_seconds(costs)
     steps = len(points)
     value = 1.0 / total           # one pose through the full 20-step schedule
@@ -214,7 +218,7 @@ def workload_config(cli, poses):
                         f"[{cfgname}], 20-step expbeta schedule",
             "poses_per_gpu": poses, "n_res": cli.n_res, "n_atoms": cli.n_atoms, "sh_lmax": cli.sh_lmax,
             "l2": "per-step working set (edge embeddings ~0.3 GB per receptor edge group and layer, operand images, "
-                  "node tensors) exceeds the 126 MB L2; no explicit flush",
+                  "node tensors) exceeds the 50 MB L2; no explicit flush",
             "warmup_executed": cli.warmup if getattr(cli, 'short_warmup', False) else max(cli.warmup, N_SCHED),
             "launch": "one CUDA-graph replay per step (diffdock_b200.sampling.GraphedSteps); the eager op-by-op step is "
                       "reported as eager_ms_per_step",
@@ -258,19 +262,6 @@ def tpconv_stream_roofline(dev, n_edges=200000):
             "edges": n_edges, "bytes_per_launch": nbytes, "ms_per_launch": ms, "traffic": None,
             "how": "standalone launches, CUDA events, weights (5.7 GB) larger than L2; the model itself runs the fully "
                    "fused kernel (see 'roofline')"}
-
-
-def _ncu_traffic():
-    """DRAM bytes per launch of the fused kernel from the committed ncu capture of this round (None if absent): the run
-    itself cannot read dram__bytes without a profiler attached."""
-    for name in ('r02m_fused_traffic.json', 'r02_fused_traffic.json'):        # newest capture first
-        p = os.path.join(ROOT, 'profiles', name)
-        if os.path.exists(p):
-            try:
-                return json.load(open(p))
-            except Exception:
-                return None
-    return None
 
 
 class Workload:
@@ -356,6 +347,25 @@ class Workload:
         return sorted(times)[len(times) // 2], times, final
 
 
+def dump_outputs(out_dir, arrays):
+    """Writes {name: array} as out_dir/<name>.npy in float32 (float64 arrays stay float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if torch.is_tensor(a) else np.asarray(a)
+        np.save(os.path.join(out_dir, f'{name}.npy'), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
+
+
+def workload_outputs(w):
+    """What the timed single-complex path hands its caller after its last step: the ligand coordinates of every pose
+    [poses, atoms, 3], and the diffusion step that produced them."""
+    torch.cuda.synchronize()
+    if w.graphed is not None:
+        pos, step = w.graphed.pos, int(w.graphed.step.item())
+    else:
+        pos, step = w.g['ligand'].pos, -1
+    return {'ligand_pos': pos.float().reshape(w.n_poses, -1, 3), 'step_index': np.array([step], dtype=np.float64)}
+
+
 def timed_steps(w, steps, warmup_steps, sync_all):
     for i in range(warmup_steps):
         w.step(i)
@@ -418,6 +428,8 @@ def run_cuda(cli):
     sync_all()
     ms = e0.elapsed_time(e1) / cli.steps
     clocks = sampler.stop() if sampler else None
+    if cli.dump_outputs and rank == 0:
+        dump_outputs(cli.dump_outputs, workload_outputs(w))
     ms_max = max_over_ranks(ms)
     value = world * cli.poses / (N_SCHED * ms_max * 1e-3)
 
@@ -492,19 +504,18 @@ def run_cuda(cli):
             alg = prof['fused_alg_flops'] / sec / 1e12
             eq_gbs = prof['fused_bytes'] / sec / 1e9
             peak_tf = pk.get('bf16_tflops_sustained', pk['bf16_tflops'])
-            ncu = _ncu_traffic()
             roof = {"bound": "hbm", "kernel": "fused_conv_kernel",
                     "achieved": eq_gbs, "peak": pk['hbm_gbs'], "unit": "GB/s", "frac": eq_gbs / pk['hbm_gbs'],
                     "peak_kind": pk_kind + " (HBM copy bandwidth, MEASURED_PEAKS.json)",
                     "definition": "SURVEY 8(d): ALGORITHMIC bytes of the tensor-product convolution (E (4 W + 16) + node "
                                   "tensors; the per-edge weights W counted as an HBM stream although the fused kernel keeps "
-                                  "them in tensor memory) / fused-kernel time; may exceed 1 because of that",
-                    "traffic": (ncu or {}).get('dram_bytes_per_launch'), "traffic_source": (ncu or {}).get('source'),
+                                  "them on chip) / fused-kernel time; may exceed 1 because of that",
                     "tensor": {"issued_TFLOPs": issued, "issued_frac_of_bf16_peak": issued / peak_tf, "bf16_peak_TFLOPs": peak_tf,
                                "algorithmic_TFLOPs": alg,
                                "algorithmic_def": "fp32 FLOPs of the reference formulation per edge: radial MLP 2 K H + 2 H W "
-                                                  "and the tensor product (SURVEY 8(d)); issued = bf16 tcgen05 FLOPs (split-bf16 "
-                                                  "x3 + bias step, 16-column K steps, N tiles trimmed to 32 columns)",
+                                                  "and the tensor product (SURVEY 8(d)); issued = bf16 wgmma FLOPs (split-bf16 "
+                                                  "x3 + bias step, 16-column K steps, every product issued 192 columns wide on "
+                                                  "64-edge tiles)",
                                "issued_over_algorithmic": issued / alg if alg else None},
                     "launches": prof['fused_launches'],
                     "timing": "CUDA-event pair per launch on the launching stream, over K eager steps after the timed region "
@@ -634,6 +645,8 @@ def run_config5(cli):
     dev_max, wall_max = float(tt[0]), float(tt[1])
     clocks = sampler.stop() if sampler else None
     checksum = float(sum(float(p.double().sum()) for p in allpos))
+    if cli.dump_outputs and rank == 0:     # final coordinates of every complex [poses, atoms_i, 3], in complex order
+        dump_outputs(cli.dump_outputs, {f'complex_{i:03d}_ligand_pos': p.float() for i, p in enumerate(allpos)})
     finite = all(bool(torch.isfinite(p).all()) for p in allpos)
     if rank == 0:
         total = n_cx * n_poses
@@ -677,6 +690,9 @@ def main():
                     help="'config5': 64 complexes x 40 poses sharded over the GPUs (strong scaling)")
     ap.add_argument('--complexes', type=int, default=64)
     ap.add_argument('--quick', action='store_true', help='skip the config-2 / CFG-L1 side measurements')
+    ap.add_argument('--dump-outputs', dest='dump_outputs', default=None, metavar='DIR',
+                    help='after the timed steps, write what the last one computed as DIR/<name>.npy (every workload '
+                         'and --impl)')
     ap.add_argument('--short-warmup', dest='short_warmup', action='store_true',
                     help='warm up exactly --warmup steps instead of a full schedule pass (runs under ncu)')
     cli = ap.parse_args()

@@ -1,4 +1,4 @@
-"""diffdock_b200 - B200-native (sm_100a) implementation of DiffDock's score-model hot path: the
+"""diffdock_b200 - H100-native (sm_90a) implementation of DiffDock's score-model hot path: the
 TensorProductConvLayer stack + translation/rotation/torsion heads, iterated by the reverse-diffusion sampler.
 
 Drop-in surface (same names/arguments as the reference):

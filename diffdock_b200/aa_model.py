@@ -4,7 +4,7 @@ Same constructor keywords, ``forward(data) -> (tr_pred, rot_pred, tor_pred, None
 effects on ``data`` (the cached receptor / atom embeddings of models/aa_model.py:319-333) as the reference class.  It is the
 coarse-grained model (diffdock_b200/cg_model.py) with a third node type - receptor atoms - and nine edge groups per
 interaction layer instead of four (three in the last layer, models/aa_model.py:401-430); every group runs on the same
-sm_100a convolution kernels through ``TensorProductConvLayer.forward_groups`` (fully fused tcgen05 kernel when the shape
+sm_90a convolution kernels through ``TensorProductConvLayer.forward_groups`` (fully fused wgmma kernel when the shape
 allows), neighbour lists come from ddb200_radius_*, spherical harmonics are evaluated in-kernel.
 
 Two reference behaviours are reproduced on purpose: the reversed groups (residue<-ligand, residue<-atom, atom<-ligand) reuse

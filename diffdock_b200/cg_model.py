@@ -2,8 +2,8 @@
 
 Same constructor keywords, ``forward(data) -> (tr_pred, rot_pred, tor_pred, sidechain_pred)`` contract, ``state_dict``
 keys and side effects on ``data`` (SURVEY.md section 8(b)); ``utils/sampling.py:116`` can call it unchanged.  What runs
-underneath is B200-native: neighbour search and the tensor-product convolutions (SH + Clebsch-Gordan contraction +
-segmented reduction + BatchNorm/residual epilogue) are hand-written sm_100a kernels behind the C ABI
+underneath is H100-native: neighbour search and the tensor-product convolutions (SH + Clebsch-Gordan contraction +
+segmented reduction + BatchNorm/residual epilogue) are hand-written sm_90a kernels behind the C ABI
 (include/diffdock_b200.h); every edge list is produced already CSR-sorted by its convolution target; the score-norm
 tables are device buffers (no host round trips for so3/torus look-ups).
 

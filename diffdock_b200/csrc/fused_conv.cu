@@ -1,24 +1,25 @@
-// Fully fused equivariant convolution for one edge group (sm_100a): radial MLP on tcgen05 + tensor-product contraction
-// straight out of tensor memory + scatter - the per-edge weight tensor [E, weight_numel] never exists in HBM.
+// Fully fused equivariant convolution for one edge group (sm_90a): radial MLP on the Hopper tensor cores (wgmma) +
+// tensor-product contraction + scatter - the per-edge weight tensor [E, weight_numel] never exists in HBM.
 //
-//   for a unit of 256 CSR-sorted edges (a CTA pair on tcgen05 cta_group::2, 128 edges = 128 TMEM lanes per CTA, persistent
-//   over units; CG = 1: one CTA per 128-edge tile):
+//   for a tile of 64 CSR-sorted edges (one CTA, persistent over tiles; warpgroup 0 multiplies, warpgroup 1 contracts):
 //     A0' = split-bf16([edge_attr (+ per-graph term) | node[tgt,:ns] | node[src,:ns]])   built in shared memory (128B swizzle)
-//     H   = relu(A0' x W1'^T)          tcgen05.mma -> TMEM -> registers -> A' image (bias folded via two constant-one columns)
+//     H   = relu(A0' x W1'^T)          wgmma -> registers -> A' image (bias folded via two constant-one columns)
 //     for every N tile (whole rows u of one path block [mul_in, mul_out], <= 192 columns):
-//        Wt = A' x W2'^T[tile]         tcgen05.mma into one of two TMEM accumulators   (B' images streamed by TMA bulk copies)
-//        consumer thread e (= TMEM lane): acc[w,k] += Wt[e, (u,w)] * z_e[u,k],   z_e[u,k] = sum_i x[src_e][u,i] M_e[i,k],
-//                                         M_e = edge_weight * coef * C . Y(vec_e)       (tcgen05.ld 32x32b.x32 + FFMA)
-//     at the end of an output irrep: sum[tgt_e, irrep] += acc  (run reduction over equal targets through shared memory, then
-//                                                              one coalesced RED.ADD per run and 32 output values)
+//        Wt = A' x W2'^T[tile]         wgmma m64nNk16 into registers (B' images streamed by TMA bulk copies through a
+//                                      4-stage ring), then stored to a padded shared-memory tile C [64][196] once the
+//                                      consumers have drained the previous one: the next tile's MMAs overlap the contraction
+//        consumer thread pair (e, half): acc[w,k] += Wt[e, (u,w)] * z_e[u,k] over its half of the 32-column chunks,
+//                                        z_e[u,k] = sum_i x[src_e][u,i] M_e[i,k],  M_e = edge_weight * coef * C . Y(vec_e)
+//     at the end of an output irrep: sum[tgt_e, irrep] += acc  (the pair's partial sums are added and runs of equal
+//                                                              targets reduced through shared memory, then one coalesced
+//                                                              RED.ADD per run and 32 output values)
 //
 // Operand layout: BOTH operand images hold each split part once - activation [hi | lo | 1 1 0..], static operand
 // [hi | lo | b_hi b_lo 0..] (2 Kp + 16 columns, Kp = K rounded up to 16).  The three products hi.hi + hi.lo + lo.hi (+ bias)
 // are formed by an MMA schedule over 16-column steps: a `hi` step of B is multiplied with the hi AND the lo columns of A (two
 // MMAs on one staged block), a `lo` step with the hi columns, the bias step with the constant-one columns.  Compared with
-// concatenating [hi | hi | lo] x [hi | lo | hi] along K this stages 5 instead of 7 k-blocks of B per tile (the kernel is
-// bound by the latency of that stream: same ring, 40 % more tensor work per staged byte), frees 32 KB of shared memory on
-// the A side and a third of the activation stores.
+// concatenating [hi | hi | lo] x [hi | lo | hi] along K this stages 5 instead of 7 k-blocks of B per tile and a third fewer
+// activation stores.
 //
 // Replaces models/tensor_layers.py:139-144 / :204-221 *including* the FCBlock at :140/:211 and the edge_attr_ assembly of
 // models/cg_model.py:342-349 (and the per-call sigma-embedding add of :298-301 through `ea_add`).
@@ -29,193 +30,55 @@
 #include <stdlib.h>
 
 #include "../../include/diffdock_b200.h"
+#include "sm90.cuh"
 
 namespace {
 
-constexpr int BM = 128, BN = 256, BK = 64;       // CTA tile; BK bf16 = one 128-byte swizzle row
-constexpr int A_KB_BYTES = BM * BK * 2;          // 16 KB
-constexpr int B_IMAGE_BYTES = BN * BK * 2;       // 32 KB: one k-block image of an N tile in global memory
-// CG = CTAs per MMA (tcgen05 cta_group): with CG = 2 a CTA pair works on 256 edges, each CTA stages only its half of the
-// rows of every B image (half the L2->smem traffic and half the B reads per SM), so the ring can be deeper.
+using namespace ddb200_sm90;
+
+constexpr int BM = 64, BK = 64;                  // CTA tile = one wgmma M; BK bf16 = one 128-byte swizzle row
+constexpr int A_KB_BYTES = BM * BK * 2;          // 8 KB
+constexpr int B_IMAGE_BYTES = 256 * BK * 2;      // 32 KB: one k-block image of an N tile in global memory
 constexpr int MAX_N = 192;                       // widest N tile of a plan (and widest hidden layer)
-template <int CG> struct Ring {
-  static constexpr int STAGES = CG == 2 ? 9 : 4;
-  static constexpr int STAGE_BYTES = MAX_N * BK * 2 / CG;     // 24 KB, or 12 KB per CTA of a pair
-};
+constexpr int STAGES = 4;
+constexpr int STAGE_BYTES = MAX_N * BK * 2;      // 24 KB: the rows of an image the MMA reads
 constexpr int MAX_KB = 5;                        // k-blocks of either operand image: 2 Kp + 16 <= 320  (Kp <= 144)
 constexpr int MAX_KA = MAX_KB;
 constexpr int OPS_PER_KB = 8;                    // MMAs that read one staged k-block of B (4 steps x up to 2 A partners)
-constexpr int THREADS = 256;
+constexpr int THREADS = 256;                     // warpgroup 0: MMA, warpgroup 1: consumers (two threads per edge)
 constexpr int MAX_TILES = 128, MAX_PATHS = 16, MTAB = 48;     // per path: dense [3][3][5] table, padded to 48 floats
 constexpr int FLUSH_LD = 33;                     // padded row of the per-warp scatter staging buffer [48][33]
+constexpr int CLD = 196;                         // row of the accumulator tile: 16-byte reads of 8 rows hit 8 bank groups
+constexpr int BAR_MMA = 1, BAR_PAIR = 2;         // named barriers: the MMA warpgroup, the two consumer warp pairs
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void mbar_wait_u32(uint32_t bar, uint32_t parity) {   // barrier given by its shared address
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the barrier at the same shared-memory offset in CTA `rank` of the cluster (release at cluster scope)
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(smem_u32(bar)), "r"(rank)
-      : "memory");
-}
-// same, without the cluster-scope release: for forwarding a completion the thread itself wrote nothing for
-// (cluster-scope release/acquire on mbarrier operations costs ~1000 clocks each, measured)
-__device__ __forceinline__ void mbar_arrive_remote_relaxed(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(smem_u32(bar)), "r"(rank)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-// exactly one lane of the (converged) warp gets true.  The single-thread instructions (bulk copies, tcgen05.mma / commit)
-// are issued under this predicate from warp-uniform loops: under `if (lane == 0)` the compiler wraps every one of them in
-// an ELECT / R2UR.BROADCAST / BRA.U.ANY loop (~95 clocks per tcgen05.mma, measured).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-template <int CG>
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-  else   // arrives on the barrier at this offset in BOTH CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-                 : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start address >> 4 in [0,14),
-// LBO (unused for swizzled K-major) = 1 in [16,30), SBO = 1024 B (8 rows x 128 B) >> 4 in [32,46), version 1 in [46,48),
-// layout type SWIZZLE_128B = 2 in [61,64).  The descriptor is passed as its low word (address field + LBO); the high word
-// is a constant, so the issuing loop only adds small offsets to one 32-bit value per operand.
-// M = 256 (pair): rows 0-127 come from the leader CTA's A image / go to its TMEM, rows 128-255 from / to its peer; each CTA
-// holds N/2 rows of B.
-constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFF) >> 4) | (1u << 16); }
-// All MMAs that read one staged k-block of B, in ONE asm block: up to OPS_PER_KB tcgen05.mma, each guarded by a predicate
-// (op word 1 == 0xFFFFFFFF: no MMA in this slot).  a[i] = low descriptor word of the A operand (absolute), w[i] = offset of
-// the B step inside the stage (16-byte units), b_base = low descriptor word of the stage.  Issued as straight-line code the
-// instruction descriptor and the accumulator address are moved to uniform registers once per k-block, and a slot costs an
-// add, two register->uniform moves and the MMA (the branchy one-MMA-per-asm form cost ~14 instructions per MMA and made
-// the issuing thread, not the tensor pipe, the limit: 76 clk per MMA measured against 87 clk of tensor work).
-template <int CG>
-__device__ __forceinline__ void umma_stage(uint32_t tmem_d, uint32_t idesc, uint32_t accum0, uint32_t b_base,
-                                           const uint32_t (&a)[OPS_PER_KB], const uint32_t (&w)[OPS_PER_KB]) {
-#define DDB200_MMA_SLOT(CGS, I, AI, WI, PACC)                                        \
-  "setp.ne.u32 q, " WI ", 0xFFFFFFFF;\n\t"                                            \
-  "add.u32 t, %3, " WI ";\n\t"                                                        \
-  "mov.b64 da, {" AI ", %4};\n\t"                                                     \
-  "mov.b64 db, {t, %4};\n\t"                                                          \
-  "@q tcgen05.mma.cta_group::" CGS ".kind::f16 [%0], da, db, %1, " PACC ";\n\t"
-#define DDB200_MMA_STAGE(CGS)                                                         \
-  asm volatile(                                                                       \
-      "{\n\t.reg .pred p0, pt, q;\n\t.reg .b64 da, db;\n\t.reg .b32 t;\n\t"           \
-      "setp.ne.b32 p0, %2, 0;\n\t"                                                    \
-      "setp.eq.u32 pt, 0, 0;\n\t"                                                     \
-      DDB200_MMA_SLOT(CGS, 0, "%5", "%13", "p0")                                      \
-      DDB200_MMA_SLOT(CGS, 1, "%6", "%14", "pt")                                      \
-      DDB200_MMA_SLOT(CGS, 2, "%7", "%15", "pt")                                      \
-      DDB200_MMA_SLOT(CGS, 3, "%8", "%16", "pt")                                      \
-      DDB200_MMA_SLOT(CGS, 4, "%9", "%17", "pt")                                      \
-      DDB200_MMA_SLOT(CGS, 5, "%10", "%18", "pt")                                     \
-      DDB200_MMA_SLOT(CGS, 6, "%11", "%19", "pt")                                     \
-      DDB200_MMA_SLOT(CGS, 7, "%12", "%20", "pt")                                     \
-      "}"                                                                             \
-      ::"r"(tmem_d), "r"(idesc), "r"(accum0), "r"(b_base), "r"(DESC_HI),              \
-        "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(a[4]), "r"(a[5]), "r"(a[6]), "r"(a[7]),   \
-        "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])   \
-      : "memory")
-  static_assert(OPS_PER_KB == 8, "umma_stage is written for 8 slots");
-  if constexpr (CG == 1) DDB200_MMA_STAGE("1"); else DDB200_MMA_STAGE("2");
-#undef DDB200_MMA_STAGE
-#undef DDB200_MMA_SLOT
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+__device__ __forceinline__ void wgmma_wait_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 __device__ __forceinline__ void put_a(unsigned char* sA, int r, int col, __nv_bfloat16 v) {
   const int kb = col >> 6, c = (col & 63) >> 3, j = col & 7;
   *reinterpret_cast<__nv_bfloat16*>(sA + (size_t)kb * A_KB_BYTES + r * 128 + ((c ^ (r & 7)) << 4) + j * 2) = v;
+}
+// columns col, col + 1 (col even) of row r
+__device__ __forceinline__ void put_a2(unsigned char* sA, int r, int col, uint32_t v) {
+  const int kb = col >> 6, c = (col & 63) >> 3, j = col & 7;
+  *reinterpret_cast<uint32_t*>(sA + (size_t)kb * A_KB_BYTES + r * 128 + ((c ^ (r & 7)) << 4) + j * 2) = v;
 }
 // 8 consecutive columns col0..col0+7 (col0 % 8 == 0) of row r = one 16-byte chunk of the swizzled image
 __device__ __forceinline__ void put_a8(unsigned char* sA, int r, int col0, const uint4& v) {
   const int kb = col0 >> 6, c = (col0 & 63) >> 3;
   *reinterpret_cast<uint4*>(sA + (size_t)kb * A_KB_BYTES + r * 128 + ((c ^ (r & 7)) << 4)) = v;
 }
+__device__ __forceinline__ void split1(float f, __nv_bfloat16& hi, __nv_bfloat16& lo) {
+  hi = __float2bfloat16(f);
+  lo = __float2bfloat16(f - __bfloat162float(hi));
+}
 // split 8 floats into bf16 hi / lo parts, packed as two 16-byte chunks
 __device__ __forceinline__ void split8(const float* f, uint4& hi, uint4& lo) {
   uint32_t h[4], l[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const __nv_bfloat16 h0 = __float2bfloat16(f[2 * i]), h1 = __float2bfloat16(f[2 * i + 1]);
-    const __nv_bfloat16 l0 = __float2bfloat16(f[2 * i] - __bfloat162float(h0));
-    const __nv_bfloat16 l1 = __float2bfloat16(f[2 * i + 1] - __bfloat162float(h1));
+    __nv_bfloat16 h0, h1, l0, l1;
+    split1(f[2 * i], h0, l0);
+    split1(f[2 * i + 1], h1, l1);
     h[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
     l[i] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
   }
@@ -225,12 +88,11 @@ __device__ __forceinline__ void split8(const float* f, uint4& hi, uint4& lo) {
 // The tail of an operand image row: zero the padding of the hi / lo sections (K..Kp), write the two constant-one columns
 // that carry the folded bias and zero the rest of their 16-column step.
 __device__ __forceinline__ void put_a_tail(unsigned char* sA, int r, int K, int Kp) {
-  const __nv_bfloat16 one = __float2bfloat16(1.0f), zero = __float2bfloat16(0.f);
+  const __nv_bfloat16 zero = __float2bfloat16(0.f);
   for (int c = K; c < Kp; ++c) { put_a(sA, r, c, zero); put_a(sA, r, Kp + c, zero); }
   const uint32_t ones = 0x3F803F80u;     // two bf16 1.0
   put_a8(sA, r, 2 * Kp, make_uint4(ones, 0u, 0u, 0u));
   put_a8(sA, r, 2 * Kp + 8, make_uint4(0u, 0u, 0u, 0u));
-  (void)one;
 }
 
 struct FusedParams {
@@ -248,31 +110,30 @@ struct FusedParams {
   const float* vec; const float* ew; int lmax;
   float* sum; int d_out; float* cnt;
   long long n_edges; const int* n_edges_dev;
-  int dbg_noload;                                    // diagnostics: skip the B copies (timing only, results garbage)
   unsigned long long* dbg;                           // optional [32] clock counters (DDB200_FUSED_DEBUG=1), else nullptr
 };
 
-// clock counters of the warp roles: compiled in only for the DBG instantiation (DDB200_FUSED_DEBUG=1)
-#define DBG_T() (DBG ? clock64() : 0ll)
-#define DBG_ADD(i, v) do { if (DBG) atomicAdd(p.dbg + (i), (unsigned long long)(v)); } while (0)
-
-// ---- consumer: one TMEM accumulator tile (ROWS rows u of a [mul_in, MULOUT] block) times z -> acc -------------------------
-// Only the first `nch` 32-column chunks hold MMA results (the last tile of a path block may be narrower than the full tile).
+// ---- consumer: this thread's half (alternate 32-column chunks) of one accumulator tile (ROWS rows u of a [mul_in, MULOUT]
+// block) times z -> acc.  Only the first `nch` chunks hold MMA results (the last tile of a path block may be narrower).
 template <int MULOUT, int DOUT, int ROWS>
-__device__ __forceinline__ void consume_tile(uint32_t taddr, int nch, const float* __restrict__ z, float* __restrict__ acc) {
+__device__ __forceinline__ void consume_tile(const float* __restrict__ crow, int nch, int half, const float* __restrict__ z,
+                                             float* __restrict__ acc) {
   constexpr int NCOL = MULOUT * ROWS;
   static_assert(NCOL % 32 == 0 && NCOL <= MAX_N, "tile width");
 #pragma unroll
   for (int c = 0; c < NCOL / 32; ++c) {
-    if (c < nch) {
-      uint32_t v[32];
-      tmem_ld32(taddr + c * 32, v);
+    if (c < nch && (c & 1) == half) {
+      float v[32];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const float4 f = reinterpret_cast<const float4*>(crow + c * 32)[q];
+        v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
+      }
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const int col = c * 32 + j, row = col / MULOUT, w = col % MULOUT;     // compile-time after unrolling
-        const float wv = __uint_as_float(v[j]);
 #pragma unroll
-        for (int k = 0; k < DOUT; ++k) acc[w * DOUT + k] = fmaf(wv, z[row * DOUT + k], acc[w * DOUT + k]);
+        for (int k = 0; k < DOUT; ++k) acc[w * DOUT + k] = fmaf(v[j], z[row * DOUT + k], acc[w * DOUT + k]);
       }
     }
   }
@@ -310,26 +171,17 @@ __device__ __forceinline__ void prefetch_x(const float* __restrict__ src, int cn
 }
 
 // z is formed from the node values prefetched during the previous tile, then the NEXT tile's values are requested, all
-// before waiting for the accumulator: the gather latency overlaps this tile's contraction
+// before waiting for the accumulator tile: the gather latency overlaps the MMAs
 template <int MULOUT, int DOUT, int ROWS>
-__device__ __forceinline__ void tile_body(uint32_t taddr, int nch, float* xn, int d_in, const float* M, float* acc,
-                                          const float* xnext, int cnt_next, int vec2, uint64_t* tfull_bar, uint32_t parity,
-                                          unsigned long long* dbg) {
+__device__ __forceinline__ void tile_body(const float* crow, int nch, int half, float* xn, int d_in, const float* M,
+                                          float* acc, const float* xnext, int cnt_next, int vec2, uint64_t* cfull,
+                                          uint32_t parity) {
   float z[ROWS * DOUT];
-  const long long t0 = dbg ? clock64() : 0ll;
   if (d_in == 1) make_z<1, DOUT, ROWS>(xn, M, z);
   else make_z<3, DOUT, ROWS>(xn, M, z);
   prefetch_x(xnext, cnt_next, vec2, xn);
-  const long long t1 = dbg ? clock64() : 0ll;
-  mbar_wait(tfull_bar, parity);
-  tc_fence_after();
-  const long long t2 = dbg ? clock64() : 0ll;
-  consume_tile<MULOUT, DOUT, ROWS>(taddr, nch, z, acc);
-  if (dbg) {
-    atomicAdd(dbg + 22, (unsigned long long)(t1 - t0));
-    atomicAdd(dbg + 23, (unsigned long long)(t2 - t1));
-    atomicAdd(dbg + 24, (unsigned long long)(clock64() - t2));
-  }
+  mbar_wait(cfull, parity);
+  consume_tile<MULOUT, DOUT, ROWS>(crow, nch, half, z, acc);
 }
 
 // MMA schedule of one staged k-block of B (4 steps of 16 columns; images [hi | lo | bias], S = Kp / 16 steps per part):
@@ -355,114 +207,160 @@ __device__ __forceinline__ void build_ops(uint32_t* ops, int S, uint32_t a_lo0) 
   }
 }
 
-template <int CG, bool DBG>
+// B stream of a CTA: per edge tile the W1' k-blocks, then every N tile's W2' k-blocks; item i goes to stage i % STAGES
+struct Stream {
+  unsigned char* sB; uint64_t* full; const int* tiles;
+  int n1, per_unit; uint32_t len;
+  __device__ __forceinline__ void issue(const FusedParams& p, uint32_t i) const {
+    if (i >= len) return;
+    const int j = (int)(i % (uint32_t)per_unit);
+    const unsigned char* src;
+    uint32_t bytes;
+    if (j < p.n_kb1) {
+      src = reinterpret_cast<const unsigned char*>(p.w1img) + (size_t)j * B_IMAGE_BYTES;
+      bytes = (uint32_t)n1 * 128u;
+    } else {                    // image (t, kb) of the W2' set lies at (t * n_kb + kb) = j - n_kb1
+      src = reinterpret_cast<const unsigned char*>(p.w2img) + (size_t)(j - p.n_kb1) * B_IMAGE_BYTES;
+      bytes = (uint32_t)tiles[((j - p.n_kb1) / p.n_kb) * 8 + 1] * 128u;
+    }
+    const uint32_t s = i % STAGES;
+    bulk_load(sB + (size_t)s * STAGE_BYTES, src, bytes, &full[s]);
+  }
+};
+
+// ---- MMA warpgroup: all k-blocks of one N tile (N = MMA width), then its epilogue: the hidden layer is
+// written back over the operand image as A' (ReLU, bf16 split), a weight tile is stored to the accumulator tile C.
+// One MMA group stays in flight while the previous k-block's stage is refilled.
+template <int N>
+__device__ __forceinline__ void mma_tile(const FusedParams& p, const Stream& st, const uint32_t* ops, int nkb, uint32_t& mc,
+                                         bool hidden, unsigned char* sA, float* sC, uint64_t* cfull, uint64_t* cempty,
+                                         uint32_t& cc, int t) {
+  float d[N / 2];
+  const uint32_t b_lo0 = gmma_desc_lo(smem_u32(st.sB));
+  for (int kb = 0; kb < nkb; ++kb, ++mc) {
+    const uint32_t s = mc % STAGES;
+    mbar_wait(&st.full[s], (mc / STAGES) & 1);
+    const uint32_t* oa = ops + kb * 2 * OPS_PER_KB;
+    const uint32_t* ob = oa + OPS_PER_KB;
+    const uint32_t b_lo = b_lo0 + s * (STAGE_BYTES >> 4);
+    uint32_t av[OPS_PER_KB], bv[OPS_PER_KB];
+#pragma unroll
+    for (int i = 0; i < OPS_PER_KB; ++i) { av[i] = oa[i]; bv[i] = ob[i] == 0xFFFFFFFFu ? ob[i] : b_lo + ob[i]; }
+    wgmma_fence();
+    Wgmma<N>::mma8(d, av, bv, (uint32_t)kb);
+    wgmma_commit();
+    if (kb > 0) {
+      wgmma_wait_one();
+      named_bar(BAR_MMA, 128);                   // every warp is done with the previous k-block's stage
+      if (t == 0) st.issue(p, mc - 1 + STAGES);
+    }
+  }
+  wgmma_wait_all();
+  wgmma_fence_regs(d);
+  named_bar(BAR_MMA, 128);
+  if (t == 0) st.issue(p, mc - 1 + STAGES);
+  const int lane = t & 31, r0 = (t >> 5) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+  if (hidden) {
+    const int K = p.H, Kp = p.Hp;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int c = 8 * j + c0, r = r0 + 8 * h;
+        __nv_bfloat16 h0, l0, h1, l1;
+        split1(fmaxf(d[4 * j + 2 * h], 0.f), h0, l0);
+        split1(fmaxf(d[4 * j + 2 * h + 1], 0.f), h1, l1);
+        if (c + 1 < K) {
+          put_a2(sA, r, c, (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16));
+          put_a2(sA, r, Kp + c, (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16));
+        } else if (c < K) {
+          put_a(sA, r, c, h0);
+          put_a(sA, r, Kp + c, l0);
+        }
+      }
+    if (t < BM) put_a_tail(sA, t, K, Kp);
+    fence_proxy_async();
+    named_bar(BAR_MMA, 128);                     // A' complete before the first weight-tile MMA reads it
+  } else {
+    mbar_wait(cempty, (cc & 1) ^ 1);             // the consumers have drained the previous tile
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<float2*>(sC + (r0 + 8 * h) * CLD + 8 * j + c0) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+    mbar_arrive(cfull);
+    ++cc;
+  }
+}
+
 __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParams p) {
-  constexpr int STAGES = Ring<CG>::STAGES, B_STAGE_BYTES = Ring<CG>::STAGE_BYTES;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  unsigned char* sA = smem;                                      // MAX_KA x 16 KB
+  unsigned char* sA = smem;                                      // MAX_KA x 8 KB
   unsigned char* sB = smem + (size_t)MAX_KA * A_KB_BYTES;        // ring of B stages
-  float* sY = reinterpret_cast<float*>(sB + STAGES * B_STAGE_BYTES);   // [9][128] spherical harmonics per consumer thread
-  float* sFlush = sY + 9 * 128;                                  // [4 warps][48][33] scatter staging
+  float* sC = reinterpret_cast<float*>(sB + STAGES * STAGE_BYTES);    // [64][CLD] accumulator tile
+  float* sY = sC + BM * CLD;                                     // [2][9][64] spherical harmonics per consumer thread
+  float* sFlush = sY + 2 * 9 * BM;                               // [4 warps][48][33] scatter staging
   float* sMtab = sFlush + 4 * 48 * FLUSH_LD;                     // [MAX_PATHS][48]
   int* sTiles = reinterpret_cast<int*>(sMtab + MAX_PATHS * MTAB);   // [MAX_TILES][8]
-  uint32_t* sOps = reinterpret_cast<uint32_t*>(sTiles + MAX_TILES * 8);   // [2][MAX_KB][2][OPS_PER_KB] MMA schedules (16 B aligned)
+  uint32_t* sOps = reinterpret_cast<uint32_t*>(sTiles + MAX_TILES * 8);   // [2][MAX_KB][2][OPS_PER_KB] MMA schedules
   uint64_t* bars = reinterpret_cast<uint64_t*>(sOps + 2 * MAX_KB * 2 * OPS_PER_KB);
-  uint64_t* full = bars;                 // B stage s has landed: this CTA's part (TMA complete_tx) and, on the leader, the peer's
-  uint64_t* empty = bars + STAGES;       // the MMAs reading stage s are done (commit; both CTAs of a pair)
-  uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = tfull + 2;          // leader: consumers of all CG CTAs have drained the accumulator
-  uint64_t* a_ready = tempty + 2;        // leader: all CG operand images hold A'
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(a_ready + 1);
+  uint64_t* full = bars;                 // B stage s has landed (TMA complete_tx)
+  uint64_t* cfull = bars + STAGES;       // C holds a weight tile (128 MMA threads arrive)
+  uint64_t* cempty = cfull + 1;          // the consumers have drained C (128 consumer threads arrive)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
   const int S1 = p.K1p >> 4, S2 = p.Hp >> 4;
   for (int i = tid; i < p.n_tiles * 8; i += THREADS) sTiles[i] = p.tiles[i];
   for (int i = tid; i < p.n_paths * MTAB; i += THREADS) sMtab[i] = p.mtab[i];
-  if (tid == 32) build_ops(sOps, S1, umma_desc_lo(smem_u32(sA)));
-  if (tid == 64) build_ops(sOps + MAX_KB * 2 * OPS_PER_KB, S2, umma_desc_lo(smem_u32(sA)));
+  if (tid == 32) build_ops(sOps, S1, gmma_desc_lo(smem_u32(sA)));
+  if (tid == 64) build_ops(sOps + MAX_KB * 2 * OPS_PER_KB, S2, gmma_desc_lo(smem_u32(sA)));
   if (tid == 0) {
-    // leader of a pair: a stage is full when its own bulk copy has landed (1 arrival + transaction bytes) AND the peer has
-    // relayed the completion of its half (1 arrival): one barrier, one wait per stage in the MMA issue loop
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], (CG == 2 && leader) ? 2 : 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tfull[b], 1); mbar_init(&tempty[b], 4 * CG); }
-    mbar_init(a_ready, 4 * CG);
+    for (int s = 0; s < STAGES; ++s) mbar_init(&full[s], 1);
+    mbar_init(cfull, 128);
+    mbar_init(cempty, 128);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {   // the same warp of both CTAs of a pair allocates (cute::TMEM::Allocator2Sm contract)
-    if constexpr (CG == 1) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // instruction descriptor: f32 accumulate, bf16 x bf16, K-major both, M = 128 * CG; | (N >> 3) << 17 per tile
-  const uint32_t idesc0 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)((BM * CG) >> 4) << 24);
+  __syncthreads();
   const int n1 = ((p.H + 15) / 16) * 16;
 
   // the edge count may live on the device (neighbour lists built without a host round trip): p.n_edges is then its bound
   long long n_edges = p.n_edges;
   if (p.n_edges_dev) { const long long nd = __ldg(p.n_edges_dev); n_edges = nd < n_edges ? (nd < 0 ? 0 : nd) : n_edges; }
   const long long n_mtiles = (n_edges + BM - 1) / BM;
-  const long long n_units = (n_mtiles + CG - 1) / CG;       // a unit = the CG edge tiles one MMA covers
-  uint32_t pc = 0, mc = 0, ma = 0, ea = 0, mtc = 0, rc = 0;
+  const long long my_units = blockIdx.x < n_mtiles ? (n_mtiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+  Stream st;
+  st.sB = sB; st.full = full; st.tiles = sTiles; st.n1 = n1;
+  st.per_unit = p.n_kb1 + p.n_tiles * p.n_kb;
+  st.len = (uint32_t)(my_units * st.per_unit);
+  // the ring runs ahead across edge tiles: the next tile's W1' blocks are requested while this one is contracted
+  if (tid == 0)
+    for (int i = 0; i < STAGES; ++i) st.issue(p, (uint32_t)i);
+  uint32_t mc = 0, cc = 0, cc_con = 0;
   long long dbg_c0 = 0;
   unsigned long long dbg_g0 = 0;
-  if (DBG && blockIdx.x == 0 && tid == 0) {      // effective SM clock of this launch: clock64 ticks per globaltimer ns
+  if (p.dbg && blockIdx.x == 0 && tid == 0) {      // effective SM clock of this launch: clock64 ticks per globaltimer ns
     dbg_c0 = clock64();
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(dbg_g0));
   }
 
-  for (long long unit = blockIdx.x / CG; unit < n_units; unit += gridDim.x / CG) {
-    const long long mt = unit * CG + rank;                   // may be one past the end for the peer: all rows invalid
-    if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-    const long long t_unit = DBG_T();
-    // The hidden layer's operand images do not depend on the unit: the producer warp requests them before taking part in the
-    // operand build, so the first MMA finds them in shared memory (their stages are free or about to be: the MMAs that read
-    // the previous unit's last stages were issued before the cluster barrier above and complete on their own).
-    if (warp == 0) {
-      const uint32_t sB0 = smem_u32(sB), full0 = smem_u32(full), empty0 = smem_u32(empty);
-      const uint32_t bytes = (uint32_t)(n1 / CG) * 128u;
-      const unsigned char* src = reinterpret_cast<const unsigned char*>(p.w1img) + (size_t)rank * bytes;
-      const int npre = p.n_kb1 < STAGES ? p.n_kb1 : STAGES;      // never more than the ring holds: nothing drains it yet
-      for (int kb = 0; kb < npre; ++kb, ++pc, src += B_IMAGE_BYTES) {
-        const uint32_t s = pc % STAGES, ph = (pc / STAGES) & 1;
-        mbar_wait_u32(empty0 + s * 8, ph ^ 1);
-        if (elect_one()) {
-          if (DBG && p.dbg_noload) mbar_arrive(&full[s]);
-          else {
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full0 + s * 8), "r"(bytes) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(sB0 + s * B_STAGE_BYTES), "l"(src), "r"(bytes), "r"(full0 + s * 8) : "memory");
-          }
-        }
-        __syncwarp();
-      }
-    }
+  for (long long mt = blockIdx.x; mt < n_mtiles; mt += gridDim.x) {
+    __syncthreads();
+    const long long t_unit = p.dbg ? clock64() : 0ll;
     // ---- A0' image: [hi | lo | 1 1 0..] of [edge_attr (+ per-graph term) | node[tgt,:ns] | node[src,:ns]] -------------
     {
       const long long e0 = mt * BM;
       const int Kin = p.K1, Kp = p.K1p;
       if (tid < BM) put_a_tail(sA, tid, Kin, Kp);
       if (((p.ne | p.ns) & 7) == 0 && ((p.ld_ea | p.ld_node) & 3) == 0) {
-        // vector path: two threads per edge row, each converting a contiguous half of the row's 8-column groups (<= 9
-        // groups = 18 independent 16-byte loads).  The row's indices (attribute row, per-graph term, both end points) are
+        // vector path: four threads per edge row, each converting a contiguous quarter of the row's 8-column groups (<= 5
+        // groups = 10 independent 16-byte loads).  The row's indices (attribute row, per-graph term, both end points) are
         // loaded once per thread, then ALL data loads of the thread are issued - including the per-graph term's - then the
-        // conversions: two dependent global-memory round trips per unit (the earlier item-strided form needed an index load
-        // per group and fetched the per-graph term inside the conversion loop: three round trips, ~14 k clocks per unit).
-        const int groups = Kin >> 3, gh = (groups + 1) >> 1;
-        constexpr int PER = 9;                            // (144 / 8 + 1) / 2: Kp <= 144 (MAX_KB k-blocks)
-        const int r = tid >> 1, g0 = (tid & 1) * gh, g1 = min(groups, g0 + gh);
+        // conversions: two dependent global-memory round trips per tile.
+        constexpr int TPR = THREADS / BM;
+        const int groups = Kin >> 3, gh = (groups + TPR - 1) / TPR;
+        constexpr int PER = (144 / 8 + TPR - 1) / TPR;      // Kp <= 144 (MAX_KB k-blocks)
+        const int r = tid / TPR, g0 = (tid % TPR) * gh, g1 = min(groups, g0 + gh);
         const long long e = e0 + r;
         const bool live = e < n_edges;
         const int ge = p.ne >> 3, gs = p.ns >> 3;           // groups of the attribute / of one node section
@@ -528,136 +426,22 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
           put_a(sA, r, Kp + k, lo);
         }
       }
-      if constexpr (CG == 2) asm volatile("fence.proxy.async;" ::: "memory");
-      else asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      fence_proxy_async();
     }
-    if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-    if (tid == 0) DBG_ADD(10, DBG_T() - t_unit);
+    __syncthreads();
 
-    if (warp == 0) {
-      // ===== operand-B producer: one image set per N tile (the W1' images were requested before the operand build) ======
-      // Only the rows the MMA reads (N of the tile) are fetched: images are row-major [256][128 B]; with a CTA pair this CTA
-      // fetches its half of them (rows [rank * N/2, (rank + 1) * N/2) feed the accumulator columns of the same range).
-      // The loop is kept lean (no divisions, 32-bit shared addresses, incremental source pointers): at ~400 clocks of MMA
-      // work per stage the producer's own instruction stream is otherwise what starves the tensor pipe.
-      {
-        const uint32_t sB0 = smem_u32(sB), full0 = smem_u32(full), empty0 = smem_u32(empty);
-        const int npre = p.n_kb1 < STAGES ? p.n_kb1 : STAGES;
-        for (int t = (npre < p.n_kb1 ? -1 : 0); t < p.n_tiles; ++t) {      // t = -1: the W1' k-blocks the ring could not take
-          const int nkb = (t < 0) ? p.n_kb1 : p.n_kb;
-          const int kb_first = (t < 0) ? npre : 0;
-          const uint32_t bytes = (uint32_t)(((t < 0) ? n1 : sTiles[t * 8 + 1]) / CG) * 128u;
-          const unsigned char* src = ((t < 0) ? reinterpret_cast<const unsigned char*>(p.w1img) + (size_t)kb_first * B_IMAGE_BYTES
-                                              : reinterpret_cast<const unsigned char*>(p.w2img) +
-                                                    (size_t)t * p.n_kb * B_IMAGE_BYTES) + (size_t)rank * bytes;
-          for (int kb = kb_first; kb < nkb; ++kb, ++pc, src += B_IMAGE_BYTES) {
-            const uint32_t s = pc % STAGES, ph = (pc / STAGES) & 1;
-            const long long t0 = DBG_T();
-            mbar_wait_u32(empty0 + s * 8, ph ^ 1);
-            if (lane == 0) DBG_ADD(5, DBG_T() - t0);
-            if (elect_one()) {
-              if (DBG && p.dbg_noload) mbar_arrive(&full[s]);
-              else {
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full0 + s * 8), "r"(bytes) : "memory");
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                             ::"r"(sB0 + s * B_STAGE_BYTES), "l"(src), "r"(bytes), "r"(full0 + s * 8) : "memory");
-              }
-            }
-            __syncwarp();
-          }
-        }
+    if (__shfl_sync(0xffffffffu, tid >> 7, 0) == 0) {     // warp-uniform for the compiler
+      // ===== MMA warpgroup: hidden layer, then every N tile.  Every product is issued MAX_N wide: the stage rows past a
+      // tile's width hold stale data whose columns are never read, and one instantiation keeps the accumulators in
+      // registers (one per width spills).
+      for (int t = -1; t < p.n_tiles; ++t) {
+        const bool hidden = t < 0;
+        mma_tile<MAX_N>(p, st, sOps + (hidden ? 0 : MAX_KB * 2 * OPS_PER_KB), hidden ? p.n_kb1 : p.n_kb, mc, hidden, sA, sC,
+                        cfull, cempty, cc, tid);
       }
-    } else if (warp == 2) {
-      // ===== L2 prefetch of the next unit's streamed inputs (edge attributes, index and vector rows) ===================
-      // The operand build of the next unit is a serial phase in which the tensor pipe idles; its loads then hit L2
-      // instead of HBM.
-      const long long nu = unit + gridDim.x / CG;
-      if (nu < n_units) {
-        const long long e0n = (nu * CG + rank) * BM;
-        for (int r = lane; r < BM; r += 32) {
-          const long long e = e0n + r;
-          if (e < n_edges) {
-            const long long er = p.perm ? (long long)__ldg(p.perm + e) : e;
-            const char* row = reinterpret_cast<const char*>(p.ea + er * p.ld_ea);
-            prefetch_l2(row);
-            if (p.ne * 4 > 128) prefetch_l2(row + 128);
-            prefetch_l2(row + p.ne * 4 - 4);
-            prefetch_l2(p.vec + 3 * er);
-          }
-        }
-        if (lane < 4 && e0n + lane * 32 < n_edges) {     // contiguous index streams: 128 x 4 B per CTA
-          prefetch_l2(p.tgt + e0n + lane * 32);
-          prefetch_l2(p.src + e0n + lane * 32);
-        }
-      }
-    } else if (warp == 3 && CG == 2) {
-      // ===== relay (peer CTA only): tell the leader's MMA thread that this CTA's half of a stage has landed ===========
-      // (a plain bulk copy can only complete_tx on a barrier of the CTA it writes to - measured: signalling the leader's
-      // barrier directly hangs - so the peer forwards the completion with a remote arrive)
-      if (!leader) {
-        const int total = p.n_kb1 + p.n_tiles * p.n_kb;
-        for (int i = 0; i < total; ++i, ++rc) {
-          const uint32_t s = rc % STAGES, ph = (rc / STAGES) & 1;
-          const long long t0 = DBG_T();
-          mbar_wait(&full[s], ph);
-          const long long t1 = DBG_T();
-          if (elect_one()) mbar_arrive_remote_relaxed(&full[s], 0);
-          __syncwarp();
-          if (lane == 0) { DBG_ADD(6, t1 - t0); DBG_ADD(7, DBG_T() - t1); }
-        }
-      }
-    } else if (warp == 1) {
-      // ===== MMA issuer (leader CTA of a pair only) ================================================================
-      if (leader) {
-        const uint32_t b_lo0 = umma_desc_lo(smem_u32(sB));
-        const uint32_t full0 = smem_u32(full);
-        const long long t_role = DBG_T();
-        long long w_te = 0, w_full = 0, w_a = 0, b_issue = 0;
-        for (int t = -1; t < p.n_tiles; ++t, ++ma) {
-          const uint32_t buf = ma & 1, aph = (ma >> 1) & 1;
-          long long t0 = DBG_T();
-          mbar_wait(&tempty[buf], aph ^ 1);
-          w_te += DBG_T() - t0;
-          tc_fence_after();
-          const uint32_t d = tmem_base + buf * BN;
-          const int nkb = (t < 0) ? p.n_kb1 : p.n_kb;
-          const int nmma = (t < 0) ? n1 : sTiles[t * 8 + 1];
-          const uint4* ops = reinterpret_cast<const uint4*>(sOps + ((t < 0) ? 0 : MAX_KB * 2 * OPS_PER_KB));
-          const uint32_t idesc = idesc0 | ((uint32_t)(nmma >> 3) << 17);
-          for (int kb = 0; kb < nkb; ++kb, ++mc) {
-            const uint32_t s = mc % STAGES, ph = (mc / STAGES) & 1;
-            t0 = DBG_T();
-            mbar_wait_u32(full0 + s * 8, ph);
-            w_full += DBG_T() - t0;
-            t0 = DBG_T();
-            tc_fence_after();
-            const uint32_t b_lo = b_lo0 + s * (B_STAGE_BYTES >> 4);
-            if (elect_one()) {
-              const uint4 a0 = ops[kb * 4], a1 = ops[kb * 4 + 1], w0 = ops[kb * 4 + 2], w1 = ops[kb * 4 + 3];
-              const uint32_t av[OPS_PER_KB] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-              const uint32_t wv[OPS_PER_KB] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-              umma_stage<CG>(d, idesc, (uint32_t)kb, b_lo, av, wv);
-              umma_commit<CG>(&empty[s]);
-              if (kb == nkb - 1) umma_commit<CG>(&tfull[buf]);
-            }
-            __syncwarp();
-            b_issue += DBG_T() - t0;
-          }
-          if (t < 0) {          // hidden layer done: wait until the consumers have rewritten the operand image(s) as A'
-            t0 = DBG_T();
-            if constexpr (CG == 2) mbar_wait_cluster(a_ready, mtc & 1); else mbar_wait(a_ready, mtc & 1);
-            w_a += DBG_T() - t0;
-            tc_fence_after();
-          }
-        }
-        if (lane == 0) {
-          DBG_ADD(0, DBG_T() - t_role); DBG_ADD(1, w_te); DBG_ADD(2, w_full); DBG_ADD(3, w_a);
-          DBG_ADD(13, b_issue); DBG_ADD(14, (long long)(3 * S1 + 1) + (long long)p.n_tiles * (3 * S2 + 1));
-        }
-      }
-    } else if (warp >= 4) {
-      // ===== consumers: thread <-> edge <-> TMEM lane ===========================================================
-      const int q = warp & 3, ct = q * 32 + lane;          // row of the edge tile
+    } else {
+      // ===== consumers: two threads per edge (warps q and q ^ 2), each contracting alternate 32-column chunks ========
+      const int q = warp & 3, half = q >> 1, ct = (q & 1) * 32 + lane;     // ct = row of the edge tile
       const long long e = mt * BM + ct;
       const bool valid = e < n_edges;
       const int src_e = valid ? __ldg(p.src + e) : 0, dst_e = valid ? __ldg(p.tgt + e) : -1;
@@ -667,74 +451,27 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
       const int key_up = __shfl_up_sync(0xffffffffu, dst_e, 1);
       const uint32_t head_mask = __ballot_sync(0xffffffffu, lane == 0 || key_up != dst_e || !valid);
       float* sF = sFlush + q * 48 * FLUSH_LD;
+      const float* sFp = sFlush + (q ^ 2) * 48 * FLUSH_LD;     // the partner warp's partial sums
+      float* sYh = sY + half * 9 * BM;
       {   // real spherical harmonics of the edge vector, component normalisation (e3nn polynomials)
         float vx = valid ? p.vec_sign * __ldg(p.vec + 3 * er) : 1.f, vy = valid ? p.vec_sign * __ldg(p.vec + 3 * er + 1) : 0.f,
               vz = valid ? p.vec_sign * __ldg(p.vec + 3 * er + 2) : 0.f;
         const float nrm = fmaxf(sqrtf(vx * vx + vy * vy + vz * vz), 1e-12f);
         vx /= nrm; vy /= nrm; vz /= nrm;
         const float s3 = 1.7320508075688772f, s5 = 2.23606797749979f, s15 = 3.872983346207417f;
-        sY[0 * 128 + ct] = 1.f;
-        sY[1 * 128 + ct] = s3 * vx; sY[2 * 128 + ct] = s3 * vy; sY[3 * 128 + ct] = s3 * vz;
-        sY[4 * 128 + ct] = s15 * vx * vz;
-        sY[5 * 128 + ct] = s15 * vx * vy;
-        sY[6 * 128 + ct] = s5 * (vy * vy - 0.5f * (vx * vx + vz * vz));
-        sY[7 * 128 + ct] = s15 * vy * vz;
-        sY[8 * 128 + ct] = 0.5f * s15 * (vz * vz - vx * vx);
+        sYh[0 * BM + ct] = 1.f;
+        sYh[1 * BM + ct] = s3 * vx; sYh[2 * BM + ct] = s3 * vy; sYh[3 * BM + ct] = s3 * vz;
+        sYh[4 * BM + ct] = s15 * vx * vz;
+        sYh[5 * BM + ct] = s15 * vx * vy;
+        sYh[6 * BM + ct] = s5 * (vy * vy - 0.5f * (vx * vx + vz * vz));
+        sYh[7 * BM + ct] = s15 * vy * vz;
+        sYh[8 * BM + ct] = 0.5f * s15 * (vz * vz - vx * vx);
       }
       const float* xrow = p.x + (long long)src_e * p.ld_x;
-      {   // hidden activations: ReLU (bias already folded), bf16 split, written back over the operand image as A'
-        const uint32_t buf = ea & 1, aph = (ea >> 1) & 1;
-        const long long t0 = DBG_T();
-        mbar_wait(&tfull[buf], aph);
-        if (tid == 128) DBG_ADD(9, DBG_T() - t0);
-        tc_fence_after();
-        const int K = p.H, Kp = p.Hp;
-        for (int c0 = 0; c0 < K; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN + c0, v);
-          if ((K & 7) == 0) {
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              const int k = c0 + 8 * g;
-              if (k < K) {
-                float f[8];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) f[j] = fmaxf(__uint_as_float(v[8 * g + j]), 0.f);
-                uint4 hi, lo;
-                split8(f, hi, lo);
-                put_a8(sA, ct, k, hi);
-                put_a8(sA, ct, Kp + k, lo);
-              }
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int k = c0 + j;
-              if (k < K) {
-                const float hval = fmaxf(__uint_as_float(v[j]), 0.f);
-                const __nv_bfloat16 hi = __float2bfloat16(hval);
-                const __nv_bfloat16 lo = __float2bfloat16(hval - __bfloat162float(hi));
-                put_a(sA, ct, k, hi);
-                put_a(sA, ct, Kp + k, lo);
-              }
-            }
-          }
-        }
-        put_a_tail(sA, ct, K, Kp);
-        if constexpr (CG == 2) asm volatile("fence.proxy.async;" ::: "memory");
-        else asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if constexpr (CG == 2) { mbar_arrive_remote_relaxed(&tempty[buf], 0); mbar_arrive_remote(a_ready, 0); }
-          else { mbar_arrive(&tempty[buf]); mbar_arrive(a_ready); }
-        }
-        ++ea;
-      }
+      const float* crow = sC + ct * CLD;
       float acc[48], xn[XN], M[9];
-      const long long t_loop = DBG_T();
       prefetch_x(xrow + sTiles[2], sTiles[3] * sTiles[4], p.x_vec2, xn);
-      for (int t = 0; t < p.n_tiles; ++t, ++ea) {
+      for (int t = 0; t < p.n_tiles; ++t, ++cc_con) {
         const int* ti = sTiles + t * 8;
         const int kind = ti[0], d_in = ti[4], out_off = ti[5], flags = ti[6];
         const int tn = (t + 1 < p.n_tiles) ? t + 1 : t;          // next tile (the last one requests nothing)
@@ -746,13 +483,12 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
         }
         // M[i,k] = edge_weight * sum_j coef*C[i,j,k] * Y[sh_off + j]  (at most 3x3 for the supported paths; row-major,
         // stride 3), rebuilt only when the tile belongs to another path than its predecessor: dense table, fully unrolled
-        const long long tm0 = DBG_T();
         if (flags & 4) {
           const float* T = sMtab + ti[7] * MTAB;
           const int sh_off = (flags >> 8) & 0xff;
           float yb[5];
 #pragma unroll
-          for (int j = 0; j < 5; ++j) yb[j] = sY[min(sh_off + j, 8) * 128 + ct];
+          for (int j = 0; j < 5; ++j) yb[j] = sYh[min(sh_off + j, 8) * BM + ct];
 #pragma unroll
           for (int ik = 0; ik < 9; ++ik) {
             float a = 0.f;
@@ -761,46 +497,34 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
             M[ik] = a * ew_e;
           }
         }
-        const uint32_t buf = ea & 1, aph = (ea >> 1) & 1;
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN;
+        const uint32_t par = cc_con & 1;
         const int nch = ti[1] >> 5;
-        const long long tm1 = DBG_T();
-        unsigned long long* dbgp = (DBG && tid == 128) ? p.dbg : nullptr;
         switch (kind) {
-          case 0: tile_body<48, 1, 4>(taddr, nch, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, &tfull[buf], aph, dbgp); break;
-          case 1: tile_body<10, 3, 16>(taddr, nch, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, &tfull[buf], aph, dbgp); break;
-          case 2: tile_body<16, 1, 8>(taddr, nch, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, &tfull[buf], aph, dbgp); break;
-          default: tile_body<4, 3, 16>(taddr, nch, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, &tfull[buf], aph, dbgp); break;
+          case 0: tile_body<48, 1, 4>(crow, nch, half, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, cfull, par); break;
+          case 1: tile_body<10, 3, 16>(crow, nch, half, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, cfull, par); break;
+          case 2: tile_body<16, 1, 8>(crow, nch, half, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, cfull, par); break;
+          default: tile_body<4, 3, 16>(crow, nch, half, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, cfull, par); break;
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if constexpr (CG == 2) mbar_arrive_remote_relaxed(&tempty[buf], 0); else mbar_arrive(&tempty[buf]);
-        }
-        const long long tm2 = DBG_T();
-        if (DBG && tid == 128) {
-          DBG_ADD(16, tm1 - tm0);
-          if (kind == 0) DBG_ADD(17, tm2 - tm1); else DBG_ADD(18, tm2 - tm1);
-          if (kind == 0) DBG_ADD(19, 1); else DBG_ADD(20, 1);
-        }
+        mbar_arrive(cempty);
         if (flags & 2) {
-          // end of an output irrep: scatter-add.  The warp's 32 x nacc partial results are transposed through shared memory
-          // (padded rows: conflict-free both ways); lane i then walks the 32 edges, summing runs of equal targets (CSR order
-          // makes them contiguous; unsorted input just yields runs of length one) and issues ONE fully coalesced RED.ADD per
-          // run for output values i = 0..31 (a second pass covers values 32..47).
+          // end of an output irrep: scatter-add.  Both warps of the pair stage their 32 x nacc partial results in shared
+          // memory (padded rows: conflict-free both ways); lane i of warp `half` then walks the 32 edges adding the two
+          // partial sums, sums runs of equal targets (CSR order makes them contiguous; unsorted input just yields runs of
+          // length one) and issues ONE fully coalesced RED.ADD per run for output value 32 half + i.
           const int nacc = (kind == 0) ? 48 : (kind == 1 ? 30 : (kind == 2 ? 16 : 12));
 #pragma unroll
           for (int i = 0; i < 48; ++i)
             if (i < nacc) sF[i * FLUSH_LD + lane] = acc[i];
-          __syncwarp();
-          for (int i0 = 0; i0 < nacc; i0 += 32) {
-            const int i = i0 + lane;
+          named_bar(BAR_PAIR + (q & 1), 64);
+          const int i = 32 * half + lane;
+          if (32 * half < nacc) {
             const bool act = i < nacc;
             const float* col = sF + (act ? i : 0) * FLUSH_LD;
+            const float* colp = sFp + (act ? i : 0) * FLUSH_LD;
             float s = 0.f;
 #pragma unroll
             for (int le = 0; le < 32; ++le) {
-              s += col[le];
+              s += col[le] + colp[le];
               if (le == 31 || ((head_mask >> (le + 1)) & 1)) {          // warp-uniform: last edge of a run
                 const int d = __shfl_sync(0xffffffffu, dst_e, le);
                 if (d >= 0 && act) atomicAdd(p.sum + (long long)d * p.d_out + out_off + i, s);
@@ -808,34 +532,23 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
               }
             }
           }
-          __syncwarp();
-          if (DBG && tid == 128) DBG_ADD(21, DBG_T() - tm2);
+          named_bar(BAR_PAIR + (q & 1), 64);
         }
       }
-      if (tid == 128) DBG_ADD(8, DBG_T() - t_loop);
-      if (p.cnt) {       // edge counts per target: one atomic per run, issued by the run's first lane
+      if (p.cnt && half == 0) {       // edge counts per target: one atomic per run, issued by the run's first lane
         const bool head = (head_mask >> lane) & 1;
         const uint32_t above = (lane == 31) ? 0u : (head_mask >> (lane + 1));
         const int run_len = above ? __ffs(above) : 32 - lane;
         if (head && valid) atomicAdd(p.cnt + dst_e, (float)run_len);
       }
     }
-    if (tid == 0) { DBG_ADD(11, DBG_T() - t_unit); DBG_ADD(12, 1); }
-    ++mtc;
+    if (p.dbg && tid == 0) { atomicAdd(p.dbg + 11, (unsigned long long)(clock64() - t_unit)); atomicAdd(p.dbg + 12, 1ull); }
   }
-  if (DBG && blockIdx.x == 0 && tid == 0) {
+  if (p.dbg && blockIdx.x == 0 && tid == 0) {
     unsigned long long g1;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g1));
-    DBG_ADD(25, clock64() - dbg_c0);
-    DBG_ADD(26, g1 - dbg_g0);
-  }
-  tc_fence_before();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    if constexpr (CG == 1)
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+    atomicAdd(p.dbg + 25, (unsigned long long)(clock64() - dbg_c0));
+    atomicAdd(p.dbg + 26, g1 - dbg_g0);
   }
 }
 
@@ -862,10 +575,9 @@ unsigned long long* fused_debug_buffer(int dev) {
 
 }  // namespace
 
-// Diagnostics (DDB200_FUSED_DEBUG=1 only): copies the 32 clock counters of the fused kernel's warp roles (current device) to
-// `out` and clears them.  [0] MMA role total, [1] wait accumulator-free, [2] wait B stage, [3] wait A', [5] producer wait
-// stage-free, [8] consumer tile loop, [9] consumer wait hidden, [10] A0 build, [11] unit total, [12] units (counted per CTA).
-// Synchronises the device.
+// Diagnostics (DDB200_FUSED_DEBUG=1 only): copies the 32 clock counters of the fused kernel (current device) to `out` and
+// clears them.  [11] clocks spent per edge tile (summed over tiles), [12] edge tiles, [25] / [26] clock64 ticks / ns of
+// CTA 0 over the launch.  Synchronises the device.
 extern "C" int ddb200_fused_debug_read(uint64_t* out) {
   int dev = 0;
   cudaGetDevice(&dev);
@@ -902,51 +614,22 @@ extern "C" int ddb200_fused_conv(const ddb200_fused_args* a, void* stream) {
   p.x = a->x; p.ld_x = a->ld_x; p.x_vec2 = (a->x_pairs_ok && (a->ld_x & 1) == 0 && (reinterpret_cast<uintptr_t>(a->x) & 7) == 0) ? 1 : 0;
   p.vec = a->edge_vec; p.ew = a->edge_weight; p.lmax = a->sh_lmax; p.sum = a->sum; p.d_out = a->d_out; p.cnt = a->cnt;
   p.n_edges = a->n_edges; p.n_edges_dev = a->n_edges_dev;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= MAX_DEVICES) return DDB200_EINVAL;
   p.dbg = fused_debug_buffer(dev);
-  static const int noload = [] { const char* e = getenv("DDB200_FUSED_NOLOAD"); return e ? atoi(e) : 0; }();
-  p.dbg_noload = p.dbg ? noload : 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long n_mtiles = (a->n_edges + BM - 1) / BM;
-  // CTA pairs (tcgen05 cta_group::2) unless disabled; every tile width of the plan (multiples of 32, hidden rounded to 16)
-  // splits into two halves of whole 8-row swizzle atoms
-  static const int pair_env = [] { const char* e = getenv("DDB200_FUSED_CTA_PAIR"); return e ? atoi(e) : 1; }();
-  const bool pair = pair_env != 0 && n_mtiles >= 2;
-  const size_t fixed = (9 * 128 + 4 * 48 * FLUSH_LD + MAX_PATHS * MTAB) * 4 + MAX_TILES * 8 * 4 +
-                       2 * MAX_KB * 2 * OPS_PER_KB * 4 + 28 * sizeof(uint64_t) + 1024;
-  const size_t smem = (size_t)MAX_KA * A_KB_BYTES + fixed +
-                      (pair ? Ring<2>::STAGES * Ring<2>::STAGE_BYTES : Ring<1>::STAGES * Ring<1>::STAGE_BYTES);
+  const size_t fixed = (BM * CLD + 2 * 9 * BM + 4 * 48 * FLUSH_LD + MAX_PATHS * MTAB) * 4 + MAX_TILES * 8 * 4 +
+                       2 * MAX_KB * 2 * OPS_PER_KB * 4 + (STAGES + 2) * sizeof(uint64_t) + 1024;
+  const size_t smem = (size_t)MAX_KA * A_KB_BYTES + (size_t)STAGES * STAGE_BYTES + fixed;
   if (smem > 227 * 1024) return DDB200_ESMEM;
   if (!g_dev[dev].attr_done) {      // the opt-in is a per-device attribute
-    cudaError_t e = cudaSuccess;
-    const void* fns[4] = {(const void*)fused_conv_kernel<1, false>, (const void*)fused_conv_kernel<2, false>,
-                          (const void*)fused_conv_kernel<1, true>, (const void*)fused_conv_kernel<2, true>};
-    for (int i = 0; i < 4 && e == cudaSuccess; ++i)
-      e = cudaFuncSetAttribute(fns[i], cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    const cudaError_t e = cudaFuncSetAttribute(fused_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     g_dev[dev].attr_done = true;
   }
-  if (!pair) {
-    const unsigned grid = (unsigned)(n_mtiles < sms ? n_mtiles : sms);
-    if (p.dbg) fused_conv_kernel<1, true><<<grid, THREADS, smem, (cudaStream_t)stream>>>(p);
-    else fused_conv_kernel<1, false><<<grid, THREADS, smem, (cudaStream_t)stream>>>(p);
-    return (int)cudaGetLastError();
-  }
-  const long long n_units = (n_mtiles + 1) / 2;
-  const long long max_pairs = sms / 2;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(2 * (n_units < max_pairs ? n_units : max_pairs)));
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t e = p.dbg ? cudaLaunchKernelEx(&cfg, fused_conv_kernel<2, true>, p)
-                        : cudaLaunchKernelEx(&cfg, fused_conv_kernel<2, false>, p);
-  return e != cudaSuccess ? (int)e : (int)cudaGetLastError();
+  const unsigned grid = (unsigned)(n_mtiles < sms ? n_mtiles : sms);
+  fused_conv_kernel<<<grid, THREADS, smem, (cudaStream_t)stream>>>(p);
+  return (int)cudaGetLastError();
 }

@@ -269,7 +269,7 @@ int ddb200_edge_embed(const float* edge_vec, const int32_t* edge_row, const floa
                       const int32_t* n_edges_dev, float* out, void* stream) {
   if (!edge_vec || !edge_row || !u || !w1_rbf || !w2 || !b2 || !rbf_offset || !out || capacity < 0) return DDB200_EINVAL;
   if (capacity == 0) return 0;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long blocks = (capacity + 127) / 128;

@@ -1,4 +1,4 @@
-// Radial-MLP output layer on the 5th-gen tensor cores (tcgen05 + TMEM), fp32-accurate via a split-bf16 product.
+// Radial-MLP output layer on the Hopper tensor cores (wgmma), fp32-accurate via a split-bf16 product.
 //
 //   W[e, n] = sum_k H[e, k] * W2[n, k] + b2[n]          (models/layers.py:10-17 last nn.Linear of FCBlock,
 //                                                         applied at models/tensor_layers.py:140,211)
@@ -6,122 +6,35 @@
 // The reference runs it as an fp32 GEMM; plain TF32/BF16 tensor-core math misses the 1e-4 score tolerance (measured
 // 2e-3 / 3e-2), so each operand is split x = hi + lo (two bf16) and the three significant products are evaluated as ONE
 // bf16 GEMM over a concatenated K axis:   A' = [hi(H) | hi(H) | lo(H)],  B' = [hi(W2) | lo(W2) | hi(W2)]   (K' = 3K, padded
-// to a multiple of 64), fp32 accumulation in TMEM.  Measured score error 2e-5.
+// to a multiple of 64), fp32 accumulation.  Measured score error 2e-5.
 //
-// CTA = 128 edges (UMMA_M = 128, cta_group::1) x all N tiles of 256 columns, persistent over edge tiles:
+// CTA = 128 edges x all N tiles of 256 columns, persistent over edge tiles:
 //   * A' tile: built in-kernel from fp32 H (split + 128B-swizzled K-major shared image, 16 KB per 64-wide k-block),
 //     resident for the whole edge tile;
 //   * B' tile: pre-split, pre-swizzled 32 KB images in global memory (one per (N tile, k-block), L2 resident), streamed
-//     by 1-D TMA bulk copies (UBLKCP) through a 3-stage mbarrier ring - no tensor maps needed;
-//   * one elected thread issues tcgen05.mma (SASS UTCHMMA) 128x256x16, 4 per k-block; tcgen05.commit frees the stage;
-//   * two 256-column TMEM accumulators: the 4 epilogue warps drain one (tcgen05.ld 32x32b.x32 -> + bias -> st.global)
-//     while the next N tile is being multiplied into the other.
+//     by 1-D TMA bulk copies through a 3-stage mbarrier ring (one producer warp) - no tensor maps needed;
+//   * two math warpgroups, 64 edge rows each, multiply every staged k-block with wgmma m64n256k16 into registers
+//     (128 fp32 accumulators per thread) and write the tile + bias straight from the accumulator fragments.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
 
 #include "../../include/diffdock_b200.h"
+#include "sm90.cuh"
 
 namespace {
 
+using namespace ddb200_sm90;
+
 constexpr int BM = 128, BN = 256, BK = 64;       // CTA tile; BK bf16 = one 128-byte swizzle row
+constexpr int WG_ROWS = 64;                      // rows of one warpgroup MMA
 constexpr int STAGES = 3;
 constexpr int A_KB_BYTES = BM * BK * 2;          // 16 KB
 constexpr int B_STAGE_BYTES = BN * BK * 2;       // 32 KB
 constexpr int MAX_KB = 7;                        // K' <= 448 (K <= 149)
-constexpr int THREADS = 256;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-// multicast variant: one L2 read lands in the same shared-memory offset of every CTA of the cluster in cta_mask, and
-// performs complete_tx on the mbarrier at the same offset in each of them
-__device__ __forceinline__ void bulk_g2s_mcast(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
-      ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(cta_mask)
-               : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// exactly one lane of the (converged) warp gets true: the single-thread instructions (bulk copies, tcgen05.mma / commit) are
-// issued under this predicate from warp-uniform loops - under `if (lane == 0)` the compiler wraps every one of them in an
-// ELECT / R2UR.BROADCAST / BRA.U.ANY loop (~95 clocks per tcgen05.mma, measured on the fused kernel)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start address >> 4 in [0,14),
-// LBO (unused for swizzled K-major) = 1 in [16,30), SBO = 1024 B (8 rows x 128 B) >> 4 in [32,46), version 1 in [46,48),
-// layout type SWIZZLE_128B = 2 in [61,64).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+constexpr int MATH_THREADS = 256;                // two warpgroups
+constexpr int THREADS = MATH_THREADS + 32;       // + the producer warp
 
 // element (row r, column col) of a K-major, 128B-swizzled operand image made of 16 KB k-blocks of 64 columns
 __device__ __forceinline__ void put_a(unsigned char* sA, int r, int col, __nv_bfloat16 v) {
@@ -148,62 +61,51 @@ struct GemmParams {
   int debug_nostore;   // profiling aid (DDB200_GEMM_NOSTORE=1): run everything but the global stores
 };
 
-template <int CL>   // thread-block cluster size: the B' stream is multicast to the CL CTAs of a cluster
+// all k-blocks of one 256-column product for this warpgroup's 64 rows: d = A'[rows] x B'^T, B' streamed through the ring
+__device__ __forceinline__ void mma_tile(float (&d)[BN / 2], uint32_t a_lo0, uint32_t b_lo0, int nkb, uint32_t& mc,
+                                         uint64_t* full, uint64_t* empty, int lane) {
+  for (int kb = 0; kb < nkb; ++kb, ++mc) {
+    const uint32_t s = mc % STAGES, ph = (mc / STAGES) & 1;
+    mbar_wait(&full[s], ph);
+    wgmma_fence();
+    const uint32_t a = a_lo0 + kb * (A_KB_BYTES >> 4), b = b_lo0 + s * (B_STAGE_BYTES >> 4);
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk)
+      Wgmma<BN>::mma(d, gmma_desc(a + kk * 2), gmma_desc(b + kk * 2), (kb | kk) != 0);
+    wgmma_commit();
+    wgmma_wait_all();
+    wgmma_fence_regs(d);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);      // this warp is done reading stage s
+  }
+}
+
 __global__ void __launch_bounds__(THREADS, 1) radial_gemm_kernel(const GemmParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  // SWIZZLE_128B operands need 1024-byte aligned tiles: align the dynamic window by hand (1 KB of slack is allocated)
-  // (offset arithmetic on the __shared__ symbol keeps the pointers in the shared address space: LDS/STS, not generic LD/ST)
+  // 128B-swizzled operands need 1024-byte aligned tiles: align the dynamic window by hand (1 KB of slack is allocated)
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  // layout: [A: n_kb x 16 KB][B ring: 3 x 32 KB][epilogue transpose buffers][barriers]
+  // layout: [A: n_kb x 16 KB][B ring: 3 x 32 KB][barriers]
+  const int n_kb_max = p.n_kb > p.n_kb1 ? p.n_kb : p.n_kb1;
   unsigned char* sA = smem;
-  unsigned char* sB = smem + (size_t)p.n_kb * A_KB_BYTES;
-  unsigned char* sStage = sB + STAGES * B_STAGE_BYTES;            // 4 epilogue warps x 32 x 33 floats (transpose buffer)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sStage + 4 * 32 * 33 * 4);
+  unsigned char* sB = smem + (size_t)n_kb_max * A_KB_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + STAGES * B_STAGE_BYTES);
   uint64_t* full = bars;               // [STAGES]
-  uint64_t* empty = bars + STAGES;     // [STAGES]
-  uint64_t* tfull = bars + 2 * STAGES; // [2]
-  uint64_t* tempty = tfull + 2;        // [2]
-  uint64_t* a_ready = tempty + 2;      // [1] hidden activations written back as the A' image (fused first layer)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(a_ready + 1);
+  uint64_t* empty = bars + STAGES;     // [STAGES]: one arrival per math warp
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CL); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tfull[b], 1); mbar_init(&tempty[b], 4); }
-    mbar_init(a_ready, 4);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], MATH_THREADS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {   // TMEM: all 512 columns (two 256-column fp32 accumulators)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CL > 1) cluster_sync_all();     // every CTA's barriers are initialised before any remote arrive / multicast
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t crank = (CL > 1) ? cluster_ctarank() : 0u;
-  constexpr uint16_t kMask = (uint16_t)((1u << CL) - 1u);
-
-  // instruction descriptor: D=f32 (bit 4), A=B=bf16 (bits 7,10), K-major A and B, N>>3 at [17,23), M>>4 at [24,29)
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
 
   const bool fuse1 = (p.h == nullptr);
-  const int n1 = ((p.K + 15) / 16) * 16;     // first-layer MMA N (hidden width rounded to the UMMA granularity)
-  const uint32_t idesc1 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n1 >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-  uint32_t mtc = 0;  // edge tiles processed by this CTA (phase of a_ready)
   const long long n_mtiles = (p.n_edges + BM - 1) / BM;
   uint32_t pc = 0;   // producer k-block counter   (stage = pc % STAGES, phase = (pc / STAGES) & 1)
   uint32_t mc = 0;   // MMA k-block counter
-  uint32_t ma = 0;   // MMA accumulator counter    (buf = ma & 1, phase = (ma >> 1) & 1)
-  uint32_t ea = 0;   // epilogue accumulator counter
 
-  // a cluster walks CL consecutive edge tiles at a time in lock step (coupled through the shared B' stream); a CTA whose
-  // tile index falls past the end still drains the pipeline on an all-zero tile
-  for (long long mt0 = (long long)(blockIdx.x / CL) * CL; mt0 < n_mtiles; mt0 += gridDim.x) {
-    const long long mt = mt0 + crank;
-    __syncthreads();   // previous tile fully drained (epilogue passed its last tmem_full => all MMAs that read A are done)
+  for (long long mt = blockIdx.x; mt < n_mtiles; mt += gridDim.x) {
+    __syncthreads();   // previous tile fully drained (every math warp passed its last MMA wait)
     // ---- build the first MMA operand image: rows = edges, cols = [hi | hi | lo], 128B-swizzled, zero padded ----------
     {
       const long long e0 = mt * BM;
@@ -234,114 +136,40 @@ __global__ void __launch_bounds__(THREADS, 1) radial_gemm_kernel(const GemmParam
         put_a(sA, r, Kin + k, hi);
         put_a(sA, r, 2 * Kin + k, lo);
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the MMA (async proxy)
+      fence_proxy_async();
     }
     __syncthreads();
 
-    if (warp == 0) {
-      // ===== B producer =====================================================================================
-      {   // warp-uniform loops, one elected lane issues
-        if (fuse1)
-          for (int kb = 0; kb < p.n_kb1; ++kb, ++pc) {
-            const uint32_t s = pc % STAGES, ph = (pc / STAGES) & 1;
-            mbar_wait(&empty[s], ph ^ 1);
-            const unsigned char* src = reinterpret_cast<const unsigned char*>(p.w1img) + (size_t)kb * B_STAGE_BYTES;
-            if (elect_one()) {
-              mbar_expect_tx(&full[s], B_STAGE_BYTES);
-              if constexpr (CL == 1) {
-                bulk_g2s(sB + (size_t)s * B_STAGE_BYTES, src, B_STAGE_BYTES, &full[s]);
-              } else if (crank == 0) {
-                bulk_g2s_mcast(sB + (size_t)s * B_STAGE_BYTES, src, B_STAGE_BYTES, &full[s], kMask);
-              }
-            }
-            __syncwarp();
-          }
-        for (int nt = 0; nt < p.n_tiles_n; ++nt)
-          for (int kb = 0; kb < p.n_kb; ++kb, ++pc) {
-            const uint32_t s = pc % STAGES, ph = (pc / STAGES) & 1;
-            mbar_wait(&empty[s], ph ^ 1);       // all CL CTAs have consumed this stage
-            const unsigned char* src =
-                reinterpret_cast<const unsigned char*>(p.bimg) + ((size_t)nt * p.n_kb + kb) * B_STAGE_BYTES;
-            if (elect_one()) {
-              mbar_expect_tx(&full[s], B_STAGE_BYTES);
-              if constexpr (CL == 1) {
-                bulk_g2s(sB + (size_t)s * B_STAGE_BYTES, src, B_STAGE_BYTES, &full[s]);
-              } else if (crank == 0) {
-                bulk_g2s_mcast(sB + (size_t)s * B_STAGE_BYTES, src, B_STAGE_BYTES, &full[s], kMask);
-              }
-            }
-            __syncwarp();
-          }
+    if (warp == MATH_THREADS / 32) {
+      // ===== B producer: warp-uniform loops, one lane issues ==============================================
+      const int total = (fuse1 ? p.n_kb1 : 0) + p.n_tiles_n * p.n_kb;
+      for (int i = 0; i < total; ++i, ++pc) {
+        const uint32_t s = pc % STAGES, ph = (pc / STAGES) & 1;
+        mbar_wait(&empty[s], ph ^ 1);
+        const int j = fuse1 ? i - p.n_kb1 : i;
+        const unsigned char* src = (j < 0) ? reinterpret_cast<const unsigned char*>(p.w1img) + (size_t)i * B_STAGE_BYTES
+                                           : reinterpret_cast<const unsigned char*>(p.bimg) + (size_t)j * B_STAGE_BYTES;
+        if (lane == 0) bulk_load(sB + (size_t)s * B_STAGE_BYTES, src, B_STAGE_BYTES, &full[s]);
+        __syncwarp();
       }
-    } else if (warp == 1) {
-      // ===== MMA issuer ======================================================================================
-      {   // warp-uniform loops, one elected lane issues
-        if (fuse1) {   // hidden = A0' x W1'^T into an accumulator buffer, then wait for the epilogue to turn it into A'
-          const uint32_t buf = ma & 1, aph = (ma >> 1) & 1;
-          mbar_wait(&tempty[buf], aph ^ 1);
-          tc_fence_after();
-          const uint32_t d = tmem_base + buf * BN;
-          for (int kb = 0; kb < p.n_kb1; ++kb, ++mc) {
-            const uint32_t s = mc % STAGES, ph = (mc / STAGES) & 1;
-            mbar_wait(&full[s], ph);
-            tc_fence_after();
-            const uint32_t a0 = smem_u32(sA + (size_t)kb * A_KB_BYTES), b0 = smem_u32(sB + (size_t)s * B_STAGE_BYTES);
-            if (elect_one()) {
+    } else {
+      // ===== math warpgroups: wgmma over this warpgroup's 64 rows, epilogue from the accumulator fragments ==========
+      const int wg = tid >> 7, t = tid & 127;
+      const int r0 = wg * WG_ROWS + (t >> 5) * 16 + (lane >> 2);   // fragment rows r0, r0 + 8 (of the CTA tile)
+      const int c0 = 2 * (lane & 3);                               // fragment columns 8 j + c0 (+ 1)
+      const uint32_t a_lo0 = gmma_desc_lo(smem_u32(sA + wg * WG_ROWS * 128));
+      const uint32_t b_lo0 = gmma_desc_lo(smem_u32(sB));
+      float d[BN / 2];
+      if (fuse1) {   // hidden = A0' x W1'^T, then + bias, ReLU, bf16 split, written back over the operand image as A'
+        mma_tile(d, a_lo0, b_lo0, p.n_kb1, mc, full, empty, lane);
+        const int K = p.K, kpad = p.n_kb * BK;
 #pragma unroll
-              for (int kk = 0; kk < BK / 16; ++kk)
-                umma_bf16(d, umma_desc(a0 + kk * 32), umma_desc(b0 + kk * 32), idesc1, (kb | kk) != 0);
-              if constexpr (CL == 1) umma_commit(&empty[s]);
-              else umma_commit_mcast(&empty[s], kMask);
-              if (kb == p.n_kb1 - 1) umma_commit(&tfull[buf]);
-            }
-            __syncwarp();
-          }
-          ++ma;
-          mbar_wait(a_ready, mtc & 1);
-          tc_fence_after();
-        }
-        for (int nt = 0; nt < p.n_tiles_n; ++nt, ++ma) {
-          const uint32_t buf = ma & 1, aph = (ma >> 1) & 1;
-          mbar_wait(&tempty[buf], aph ^ 1);
-          tc_fence_after();
-          const uint32_t d = tmem_base + buf * BN;
-          for (int kb = 0; kb < p.n_kb; ++kb, ++mc) {
-            const uint32_t s = mc % STAGES, ph = (mc / STAGES) & 1;
-            mbar_wait(&full[s], ph);
-            tc_fence_after();
-            const uint32_t a0 = smem_u32(sA + (size_t)kb * A_KB_BYTES), b0 = smem_u32(sB + (size_t)s * B_STAGE_BYTES);
-            if (elect_one()) {
+        for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-              for (int kk = 0; kk < BK / 16; ++kk)
-                umma_bf16(d, umma_desc(a0 + kk * 32), umma_desc(b0 + kk * 32), idesc, (kb | kk) != 0);
-              if constexpr (CL == 1) umma_commit(&empty[s]);     // stage free once these MMAs have read it
-              else umma_commit_mcast(&empty[s], kMask);          // ... signalled to every CTA of the cluster
-              if (kb == p.n_kb - 1) umma_commit(&tfull[buf]);    // accumulator complete
-            }
-            __syncwarp();
-          }
-        }
-      }
-    } else if (warp >= 4) {
-      // ===== epilogue: TMEM -> registers -> smem transpose -> + bias -> coalesced global stores ====================
-      // (a thread owns one accumulator row; storing rows directly would scatter 16-byte pieces over 32 rows per
-      //  instruction, so each 32x32 block is transposed through a padded shared buffer and written as 128-byte rows)
-      const int q = warp & 3;                     // TMEM lane quadrant this warp may access
-      float* stg = reinterpret_cast<float*>(sStage) + (size_t)q * 32 * 33;
-      const long long e_base = mt * BM + q * 32;
-      if (fuse1) {   // hidden activations: + bias, ReLU, bf16 split, written back over the operand image as A'
-        const uint32_t buf = ea & 1, aph = (ea >> 1) & 1;
-        mbar_wait(&tfull[buf], aph);
-        tc_fence_after();
-        const int r = q * 32 + lane, K = p.K, kpad = p.n_kb * BK;
-        for (int c0 = 0; c0 < K; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN + c0, v);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int k = c0 + j;
+          for (int h = 0; h < 4; ++h) {
+            const int k = 8 * j + c0 + (h & 1), r = r0 + 8 * (h >> 1);
             if (k < K) {
-              const float hval = fmaxf(__uint_as_float(v[j]) + __ldg(p.b1 + k), 0.f);
+              const float hval = fmaxf(d[4 * j + h] + __ldg(p.b1 + k), 0.f);
               const __nv_bfloat16 hi = __float2bfloat16(hval);
               const __nv_bfloat16 lo = __float2bfloat16(hval - __bfloat162float(hi));
               put_a(sA, r, k, hi);
@@ -349,55 +177,28 @@ __global__ void __launch_bounds__(THREADS, 1) radial_gemm_kernel(const GemmParam
               put_a(sA, r, 2 * K + k, lo);
             }
           }
+        for (int idx = t; idx < WG_ROWS * (kpad - 3 * K); idx += 128) {
+          const int r = wg * WG_ROWS + idx / (kpad - 3 * K), col = 3 * K + idx % (kpad - 3 * K);
+          put_a(sA, r, col, __float2bfloat16(0.f));
         }
-        for (int col = 3 * K; col < kpad; ++col) put_a(sA, r, col, __float2bfloat16(0.f));
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) { mbar_arrive(&tempty[buf]); mbar_arrive(a_ready); }
-        ++ea;
+        fence_proxy_async();
+        named_bar(1 + wg, 128);       // this warpgroup's rows of A' are complete
       }
-      for (int nt = 0; nt < p.n_tiles_n; ++nt, ++ea) {
-        const uint32_t buf = ea & 1, aph = (ea >> 1) & 1;
-        mbar_wait(&tfull[buf], aph);
-        tc_fence_after();
-        const int nrow = (int)((p.n_edges - e_base) < 32 ? (p.n_edges - e_base) : 32);
-        float* obase = p.out + e_base * p.ldo + (long long)nt * BN + lane;
-        const float* bbase = p.bias + (long long)nt * BN + lane;
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-          uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN + c * 32, v);
+      const long long e_a = mt * BM + r0, e_b = e_a + 8;
+      for (int nt = 0; nt < p.n_tiles_n; ++nt) {
+        mma_tile(d, a_lo0, b_lo0, p.n_kb, mc, full, empty, lane);
+        if (p.debug_nostore) continue;
+        const float* bias = p.bias + (long long)nt * BN + c0;
+        float* oa = p.out + e_a * p.ldo + (long long)nt * BN + c0;
+        float* ob = oa + 8 * p.ldo;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) stg[lane * 33 + j] = __uint_as_float(v[j]);
-          __syncwarp();
-          const float b = __ldg(bbase + c * 32);
-          float* o = obase + c * 32;
-          if (p.debug_nostore) {
-            float acc = 0.f;
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) acc += stg[rr * 33 + lane] + b;
-            if (acc == 1.2345e-30f) o[0] = acc;
-          } else if (nrow == 32) {
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) o[(long long)rr * p.ldo] = stg[rr * 33 + lane] + b;
-          } else {
-            for (int rr = 0; rr < nrow; ++rr) o[(long long)rr * p.ldo] = stg[rr * 33 + lane] + b;
-          }
-          __syncwarp();
+        for (int j = 0; j < BN / 8; ++j) {
+          const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j));
+          if (e_a < p.n_edges) *reinterpret_cast<float2*>(oa + 8 * j) = make_float2(d[4 * j] + b.x, d[4 * j + 1] + b.y);
+          if (e_b < p.n_edges) *reinterpret_cast<float2*>(ob + 8 * j) = make_float2(d[4 * j + 2] + b.x, d[4 * j + 3] + b.y);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty[buf]);
       }
     }
-    ++mtc;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CL > 1) cluster_sync_all();     // nobody leaves while a peer may still signal its barriers
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
   }
 }
 
@@ -405,41 +206,20 @@ __global__ void __launch_bounds__(THREADS, 1) radial_gemm_kernel(const GemmParam
 
 static int launch_radial(GemmParams& p, void* stream) {
   const int n_kb_max = p.n_kb > p.n_kb1 ? p.n_kb : p.n_kb1;
-  const size_t smem = (size_t)n_kb_max * A_KB_BYTES + STAGES * B_STAGE_BYTES + 4 * 32 * 33 * 4 + 16 * sizeof(uint64_t) + 1024;
+  const size_t smem = (size_t)n_kb_max * A_KB_BYTES + STAGES * B_STAGE_BYTES + 2 * STAGES * sizeof(uint64_t) + 1024;
   { const char* ns = getenv("DDB200_GEMM_NOSTORE"); p.debug_nostore = (ns && ns[0] == '1') ? 1 : 0; }
-  static int cluster = -1;
-  if (cluster < 0) {
-    const char* e = getenv("DDB200_GEMM_CLUSTER");
-    cluster = e ? atoi(e) : 1;
-    if (cluster != 1 && cluster != 2 && cluster != 4) cluster = 1;
-    cudaError_t err = cudaFuncSetAttribute(radial_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (err == cudaSuccess) err = cudaFuncSetAttribute(radial_gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (err == cudaSuccess) err = cudaFuncSetAttribute(radial_gemm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (err != cudaSuccess) { cluster = -1; return (int)err; }
+  static bool attr_done = false;
+  if (!attr_done) {
+    cudaError_t err = cudaFuncSetAttribute(radial_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (err != cudaSuccess) return (int)err;
+    attr_done = true;
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long n_mtiles = (p.n_edges + BM - 1) / BM;
-  const int cl = (n_mtiles >= 2 * cluster) ? cluster : 1;
-  long long grid = (n_mtiles + cl - 1) / cl * cl;
-  const long long cap = (long long)(sms / cl) * cl;
-  if (grid > cap) grid = cap;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t le;
-  if (cl == 1) le = cudaLaunchKernelEx(&cfg, radial_gemm_kernel<1>, p);
-  else if (cl == 2) le = cudaLaunchKernelEx(&cfg, radial_gemm_kernel<2>, p);
-  else le = cudaLaunchKernelEx(&cfg, radial_gemm_kernel<4>, p);
-  if (le != cudaSuccess) return (int)le;
+  const unsigned grid = (unsigned)(n_mtiles < sms ? n_mtiles : sms);
+  radial_gemm_kernel<<<grid, THREADS, smem, (cudaStream_t)stream>>>(p);
   return (int)cudaGetLastError();
 }
 

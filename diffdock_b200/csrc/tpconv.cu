@@ -1,4 +1,4 @@
-// Fused tensor-product graph convolution for sm_100a (B200).
+// Fused tensor-product graph convolution for sm_90a (H100).
 //
 // One warp owns a run of 32 consecutive edges (edges are CSR-sorted by destination).  For every edge it
 //   1. gathers the source node's irreps row (L2-resident) into shared memory,
@@ -507,7 +507,7 @@ static int plan_smem(ddb200_tp_table* t) {
 
 extern "C" {
 
-const char* ddb200_version(void) { return "diffdock_b200 0.1.0 sm_100a"; }
+const char* ddb200_version(void) { return "diffdock_b200 0.1.0 sm_90a"; }
 
 int ddb200_tp_table_create(const int32_t* ib, int n_ints, const float* fb, int n_floats, ddb200_tp_table** out) {
   if (!ib || !fb || !out || n_ints < HDR) return DDB200_EINVAL;
@@ -566,7 +566,7 @@ int ddb200_tpconv_accumulate(const ddb200_tp_table* t, const float* x, int64_t x
   p.iblob = t->d_iblob; p.fblob = t->d_fblob; p.n_ints = t->n_ints; p.n_terms = t->n_terms;
   p.stages = t->stages; p.warps = t->warps; p.warp_floats = t->warp_floats; p.stage_floats = t->hdr[14];
   p.warp_base_off = t->warp_base_off;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long units = (n_edges + ERUN - 1) / ERUN;
@@ -584,7 +584,7 @@ int ddb200_tpconv_finalize(const float* sum, const float* cnt, int64_t n_rows, i
   if (n_rows == 0) return 0;
   const long long total = n_rows * (long long)d_out;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   tpconv_finalize_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(sum, cnt, n_rows, d_out, mean, bn_scale,
                                                                             bn_shift, residual, res_stride, res_dim, out);
   return (int)cudaGetLastError();

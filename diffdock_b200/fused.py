@@ -2,16 +2,16 @@
 Replaces, per edge group, the reference's edge_attr_ assembly (models/cg_model.py:342-349), the radial FCBlock
 (models/layers.py:10-17 at models/tensor_layers.py:140,211) and the tensor product + scatter (models/tensor_layers.py:139-144,204-221).
 
-The fused kernel computes, for a tile of 128 edges, the radial MLP on the tcgen05 tensor cores and contracts the resulting
-per-edge tensor-product weights with the edge's irreps *straight out of tensor memory* - the ``[E, weight_numel]`` weight
+The fused kernel computes, for a tile of 64 edges, the radial MLP on the Hopper tensor cores (wgmma) and contracts the resulting
+per-edge tensor-product weights with the edge's irreps *straight out of an on-chip accumulator tile* - the ``[E, weight_numel]`` weight
 tensor (11-28 KB per edge) never exists in HBM.  To make that possible the weight columns are cut into N tiles that hold
 whole rows ``u`` of one path block ``[mul_in, mul_out]``:
 
     (mul_out, 2l_out+1) = (48, 1): 4 rows x 48 columns = 192        (10, 3): 16 rows x 10 columns = 160
     (16, 1): 8 x 16 = 128                                            (4, 3): 16 x 4 = 64
 
-so that a consumer thread (one edge = one TMEM lane) knows at compile time which register of its accumulator every
-TMEM column feeds.  This module builds, from a ``TpTable`` and the radial MLP's second Linear:
+so that a consumer thread (one edge = one accumulator row) knows at compile time which register of its accumulator every
+accumulator column feeds.  This module builds, from a ``TpTable`` and the radial MLP's second Linear:
   * the tile table (int32 [T, 8]) and one dense Clebsch-Gordan table per path ([3][3][5] floats: coef * C[i, j, k]),
   * the pre-split, pre-swizzled bf16 operand images of W2 per tile (rows permuted into tile order, zero padded), with the
     bias folded in as two extra K columns (hi, lo) that multiply constant-one columns of the activation operand.
@@ -109,7 +109,7 @@ class FusedPlan:
             kind, rows_per = CONSUMER_KINDS[(p.mul_out, d_out)]
             for u0 in range(0, p.mul_in, rows_per):
                 nrow = min(rows_per, p.mul_in - u0)
-                # MMA width: the valid columns rounded up to whole 32-column TMEM chunks (columns beyond are never read)
+                # tile width: the valid columns rounded up to whole 32-column chunks (columns beyond are never read)
                 n_mma = min(rows_per * p.mul_out, (nrow * p.mul_out + 31) // 32 * 32)
                 first = group_prev != p.i_out
                 group_prev = p.i_out
@@ -141,10 +141,10 @@ class FusedPlan:
         self.mtab = torch.as_tensor(mtab, device=dev).contiguous()
         # 8-byte gathers of the node values are possible when every tile's offset and value count is even
         self.x_pairs_ok = int(all(t[2] % 2 == 0 and (t[3] * t[4]) % 2 == 0 for t in tiles))
-        # bf16 tensor-core FLOPs issued per 128-edge tile (split-bf16 x3 + bias step, 16-column steps, trimmed N tiles)
+        # bf16 tensor-core FLOPs issued per 64-edge tile (split-bf16 x3 + bias step, 16-column steps; the kernel issues every
+        # product 192 columns wide)
         s2, s1 = 3 * (_pad16(H) // 16) + 1, 3 * (_pad16(K1) // 16) + 1
-        n1 = (H + 15) // 16 * 16
-        self.mma_flops_per_tile = 2 * 128 * 16 * (n1 * s1 + sum(t[1] for t in tiles) * s2)
+        self.mma_flops_per_tile = 2 * 64 * 16 * 192 * (s1 + len(tiles) * s2)
         # algorithmic FLOPs per edge of the same work (fp32 radial MLP + tensor-product contraction, SURVEY 8(d))
         self.alg_flops_per_edge = 2 * K1 * H + 2 * H * table.weight_numel + sum(
             2 * p.mul_in * p.mul_out * (2 * p.l_out + 1) + 2 * p.mul_in * (2 * p.l_in + 1) * (2 * p.l_sh + 1) * (2 * p.l_out + 1)
@@ -214,7 +214,7 @@ def fused_conv(plan: FusedPlan, edge_attr, node, ns, tgt32, src32, x, edge_vec, 
         PROFILE.fused_pairs.append((e0, e1))
         PROFILE.fused_bytes += n_live * (4 * t.weight_numel + 12 + 4) + 4 * (sum_buf.shape[0] + 1) + \
             4 * x.shape[0] * t.d_in + 4 * sum_buf.shape[0] * t.d_out
-        PROFILE.fused_flops += ((n_live + 127) // 128) * plan.mma_flops_per_tile
+        PROFILE.fused_flops += ((n_live + 63) // 64) * plan.mma_flops_per_tile
         PROFILE.fused_alg_flops += n_live * plan.alg_flops_per_edge
     PROFILE.all_launches += 1
     _lib.check(rc, 'ddb200_fused_conv')

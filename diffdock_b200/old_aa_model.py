@@ -5,9 +5,9 @@ model) and ``utils/sampling.py:208-227`` calls once per batch of final poses (SU
 Same constructor keywords, ``forward(data) -> confidence [B]`` (``[B, 2]`` with affinity_prediction) and ``state_dict`` keys
 as the reference class for: confidence_mode=True, use_old_atom_encoder=True (the only encoder the reference class can be
 built with - its new AtomEncoder rejects the ``lm_embedding_type`` keyword, models/old_aa_model.py:71), one noise schedule,
-parallel=1.  Three node types and nine convolutions per interaction layer (:105-121, :229-266), all on the same sm_100a
+parallel=1.  Three node types and nine convolutions per interaction layer (:105-121, :229-266), all on the same sm_90a
 kernels as the score model: neighbour lists from ddb200_radius_*, spherical harmonics evaluated in-kernel from the edge
-vectors, OldTensorProductConvLayer on the fully fused tcgen05 kernel when its shapes allow.  The reversed directions
+vectors, OldTensorProductConvLayer on the fully fused wgmma kernel when its shapes allow.  The reversed directions
 (atom<-ligand, residue<-ligand, residue<-atom) reuse the forward edge attributes AND the forward vector's harmonics, as the
 reference does (:246-266).
 

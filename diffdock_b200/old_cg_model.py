@@ -4,8 +4,8 @@ model ``utils/sampling.py:208-227`` calls once per batch of final poses (SURVEY.
 Same constructor keywords, ``forward(data) -> confidence [B]`` (``[B, 2]`` with affinity_prediction) and ``state_dict``
 keys as the reference class for: confidence_mode=True, use_old_atom_encoder=True (the only encoder the reference class
 can be built with - its new AtomEncoder rejects the ``lm_embedding_type`` keyword, models/old_cg_model.py:63-66), no
-miscellaneous atoms, one noise schedule.  The convolutions are the same sm_100a kernels as the score model's: every
-OldTensorProductConvLayer call goes through the fully fused tcgen05 kernel (csrc/fused_conv.cu) when its shapes allow,
+miscellaneous atoms, one noise schedule.  The convolutions are the same sm_90a kernels as the score model's: every
+OldTensorProductConvLayer call goes through the fully fused wgmma kernel (csrc/fused_conv.cu) when its shapes allow,
 neighbour lists come from ddb200_radius_*, spherical harmonics are evaluated in-kernel from the edge vectors.
 
 CUDA only, inference only.  No CPU fallback.

@@ -1,7 +1,7 @@
 """Host side of the tensor-core radial GEMM (csrc/radial_gemm.cu): operand preparation and the launch wrapper.
 
 The last Linear of the radial MLP (models/layers.py:16; ``[E, 3ns] x [3ns, weight_numel]``, 2 MFLOP per edge) runs as a
-split-bf16 tcgen05 GEMM.  The static operand W2 is split ``W2 = hi + lo`` (bf16 each), concatenated along K as
+split-bf16 wgmma GEMM.  The static operand W2 is split ``W2 = hi + lo`` (bf16 each), concatenated along K as
 ``[hi | lo | hi]`` to pair with the in-kernel ``[hi | hi | lo]`` split of the activations, zero-padded to 256-row N tiles
 and 64-column k-blocks, and stored as the exact 128B-swizzled shared-memory images the MMA consumes, so the kernel
 streams them with plain 1-D TMA bulk copies.

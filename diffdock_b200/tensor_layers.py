@@ -1,6 +1,6 @@
 """Drop-in for the reference's ``models/tensor_layers.py``: same class name, constructor keywords, ``forward``
 signature and ``state_dict`` keys (``fc.{g}.{0,3}.weight/bias``, ``batch_norm.{weight,bias,running_mean,running_var}``),
-with the convolution executed by the fused sm_100a kernel (csrc/tpconv.cu) instead of
+with the convolution executed by the fused sm_90a kernel (csrc/tpconv.cu) instead of
 e3nn + torch_scatter (models/tensor_layers.py:125-231,309-335).
 
 Inference only (eval-mode BatchNorm, dropout = identity); CUDA only - there is no CPU fallback.
@@ -199,13 +199,13 @@ class TensorProductConvLayer(nn.Module):
 
     def _edge_weights_fused(self, fc, table, ea, node, ns, tgt32, src32):
         """Per-edge TP weights from the raw pieces: [ea | node[tgt,:ns] | node[src,:ns]] -> Linear -> ReLU -> Linear, all
-        inside ddb200_radial_mlp (split-bf16 tcgen05 GEMMs; no concatenated edge_attr_, no hidden tensor in HBM)."""
+        inside ddb200_radial_mlp (split-bf16 wgmma GEMMs; no concatenated edge_attr_, no hidden tensor in HBM)."""
         img1, b1, img2, b2p, nt = self._fused_images(fc, table)
         return radial.radial_mlp(ea, node, ns, tgt32, src32, img1, b1, fc[0].out_features, img2, b2p, nt)
 
     def _edge_weights(self, fc, table, edge_attr):
         """Radial MLP -> per-edge tensor-product weights [E, >= weight_numel_padded] in the kernel's row layout.
-        The last (dominant) Linear runs on the tcgen05 tensor cores as a split-bf16 GEMM (csrc/radial_gemm.cu);
+        The last (dominant) Linear runs on the Hopper tensor cores (wgmma) as a split-bf16 GEMM (csrc/radial_gemm.cu);
         DDB200_RADIAL_GEMM=cublas selects the plain fp32 library GEMM instead."""
         h = edge_attr
         for m in list(fc)[:-1]:

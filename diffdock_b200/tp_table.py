@@ -146,7 +146,7 @@ def _faster_paths(ins, shs, outs):
 
 
 def build_table(in_irreps, sh_irreps, out_irreps, kind='fctp', sh_from_vector=True, stage_floats=None) -> TpTable:
-    if stage_floats is None:   # TMA chunk size: 3 KB measured best on B200 (16 warps x 2 stages), see profiles/
+    if stage_floats is None:   # TMA chunk size: 3 KB (16 warps x 2 stages)
         stage_floats = int(os.environ.get('DDB200_TPCONV_STAGE_FLOATS', 768))
     ins, shs, outs = parse_irreps(in_irreps), parse_irreps(sh_irreps), parse_irreps(out_irreps)
     if kind == 'fctp':

@@ -1,7 +1,7 @@
 """Model factory: drop-in for ``utils/utils.py:get_model`` (the call inference.py:201-211 / evaluate.py use to build the score
 and confidence models from a ``model_parameters.yml`` namespace).  Same signature, same mapping from the training flags to
 constructor keywords - including the flags older checkpoints' yml files do not contain, which fall back to the reference's
-defaults - but the classes are the B200-native ones:
+defaults - but the classes are the H100-native ones:
 
     old=False : diffdock_b200.cg_model.CGModel       / diffdock_b200.aa_model.AAModel        (``all_atoms``)
     old=True  : diffdock_b200.old_cg_model.CGOldModel / diffdock_b200.old_aa_model.AAOldModel

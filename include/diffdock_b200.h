@@ -1,5 +1,5 @@
 /*
- * diffdock_b200 - C ABI of the B200-native DiffDock score-model hot path.
+ * diffdock_b200 - C ABI of the H100-native (sm_90a) DiffDock score-model hot path.
  *
  * The reference (gcorso/DiffDock @ b4704d9) is pure Python: it has no FFI of its own.  Each entry point below
  * replaces the op sequence of the cited reference lines; the Python host code in diffdock_b200/ binds them with
@@ -26,7 +26,7 @@ extern "C" {
 #define DDB200_ETABLE (-2) /* malformed tensor-product table blob                    */
 #define DDB200_ESMEM  (-3) /* table needs more shared memory than one SM offers      */
 
-/* library / build information: "diffdock_b200 <version> sm_100a" */
+/* library / build information: "diffdock_b200 <version> sm_90a" */
 const char* ddb200_version(void);
 
 /* ---------------------------------------------------------------------------------------------------------------
@@ -172,7 +172,7 @@ int ddb200_edge_embed(const float* edge_vec, const int32_t* edge_row, const floa
                       const int32_t* n_edges_dev, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Radial-MLP output layer on tcgen05 tensor cores:  out[e, n] = sum_k h[e, k] * W2[n, k] + bias[n], fp32-accurate
+ * Radial-MLP output layer on the Hopper tensor cores (wgmma):  out[e, n] = sum_k h[e, k] * W2[n, k] + bias[n], fp32-accurate
  * through a split-bf16 (hi/lo) product evaluated as one bf16 GEMM over K' = 3K.
  * h [n_edges, ldh] fp32 (K <= 149); b_images: bf16, [n_tiles_n][ceil(3K/64)][256 rows][64] pre-split
  * ([hi | lo | hi] of W2 rows, zero padded) and 128B-swizzled shared-memory images built by
@@ -187,7 +187,7 @@ int ddb200_radial_gemm(const float* h, int64_t ldh, int64_t n_edges, int K, cons
  * Whole radial MLP of one edge group in one kernel (FCBlock with two Linear layers and ReLU):
  *   a[e, :] = [edge_attr[e, :ne] | node[tgt[e], :ns] | node[src[e], :ns]]            (the torch.cat / gathers of
  *                                                                                    models/cg_model.py:342-349; ns = 0: none)
- *   h       = relu(a @ W1^T + b1)            (hidden units, also a split-bf16 tcgen05 GEMM, kept on chip)
+ *   h       = relu(a @ W1^T + b1)            (hidden units, also a split-bf16 wgmma GEMM, kept on chip)
  *   out     = h @ W2^T + b2                  (as ddb200_radial_gemm)
  * w1_images: build_b_images(W1 [hidden, ne + 2 ns]) (one N tile), w2_images / b2 / n_tiles_n / out / ldo as above.
  * Replaces: models/layers.py:10-17 (FCBlock, tp_weights_layers == 2) and the edge_attr_ assembly feeding it.
@@ -199,7 +199,7 @@ int ddb200_radial_mlp(const float* edge_attr, int64_t ld_ea, int ne, const float
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Fully fused convolution of one edge group: radial MLP (as ddb200_radial_mlp) whose output tiles are contracted with the
- * edge irreps straight out of tensor memory and scatter-added - the [E, weight_numel] weights never reach HBM.
+ * edge irreps from an on-chip accumulator tile and scatter-added - the [E, weight_numel] weights never reach HBM.
  *   r = edge_perm ? edge_perm[e] : e                                      (row of the per-edge input arrays)
  *   a = [edge_attr[r] (+ ea_add[ea_add_idx[e]]) | node[tgt[e], :ns] | node[src[e], :ns]]
  *   sum[tgt[e], :] += TP(x[src[e], :], Y(vec_sign * edge_vec[r]), FCBlock(a)) * edge_weight[r]
@@ -235,11 +235,10 @@ typedef struct ddb200_fused_args {
 } ddb200_fused_args;
 
 int ddb200_fused_conv(const ddb200_fused_args* args, void* stream);
-/* Execution: CTA pairs on tcgen05 cta_group::2 (256 edges per MMA, each CTA stages half of every weight image);
- * DDB200_FUSED_CTA_PAIR=0 selects the single-CTA kernel. */
+/* Execution: one CTA per SM, persistent over tiles of 64 edges; one warpgroup issues wgmma, one contracts. */
 
 /* Diagnostics, no reference counterpart: with DDB200_FUSED_DEBUG=1 in the environment the fused kernel accumulates clock
- * counters per warp role; this copies the 32 counters to `out` (host, uint64_t[32]) and clears them.  DDB200_EINVAL when disabled. */
+ * counters per edge tile; this copies the 32 counters to `out` (host, uint64_t[32]) and clears them.  DDB200_EINVAL when disabled. */
 int ddb200_fused_debug_read(uint64_t* out);
 
 /* ---------------------------------------------------------------------------------------------------------------

@@ -32,7 +32,7 @@ def test_all_atom_score_model_matches_reference_fixture(built_lib, idx):
 
 
 def test_all_atom_score_model_full_width_matches_oracle(built_lib):
-    """ns=48, nv=10: all nine groups on the fully fused tcgen05 kernel."""
+    """ns=48, nv=10: all nine groups on the fully fused wgmma kernel."""
     from oracle.aa_model import AAModel as OModel
     from oracle.diffusion import set_time as o_set_time, t_to_sigma as o_t2s
     from oracle.layers import get_timestep_embedding as o_temb

@@ -30,7 +30,7 @@ def test_confidence_matches_reference_fixture(built_lib, idx):
 
 
 def test_confidence_full_width_matches_oracle(built_lib):
-    """DiffDock-L-sized widths (ns=48, nv=10: the fully fused tcgen05 path) on a 60-residue complex, against the oracle."""
+    """DiffDock-L-sized widths (ns=48, nv=10: the fully fused wgmma path) on a 60-residue complex, against the oracle."""
     from oracle.diffusion import set_time as o_set_time, t_to_sigma as o_t2s
     from oracle.layers import get_timestep_embedding as o_temb
     from oracle.old_cg_model import CGOldModel as OModel
@@ -124,7 +124,7 @@ def test_all_atom_confidence_matches_reference_fixture(built_lib, idx):
 
 
 def test_all_atom_confidence_full_width_matches_oracle(built_lib):
-    """DiffDock-L-sized widths (ns=48, nv=10: the fully fused tcgen05 path for all nine convolutions) vs the oracle."""
+    """DiffDock-L-sized widths (ns=48, nv=10: the fully fused wgmma path for all nine convolutions) vs the oracle."""
     from oracle.diffusion import set_time as o_set_time, t_to_sigma as o_t2s
     from oracle.layers import get_timestep_embedding as o_temb
     from oracle.old_aa_model import AAOldModel as OModel

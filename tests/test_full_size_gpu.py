@@ -3,7 +3,7 @@ properties - the CPU oracle cannot run this size in seconds:
   * SE(3) equivariance: rotating + translating every complex rotates the translation / rotation scores and leaves the torsion
     scores unchanged;
   * pose permutation: reversing the order of the poses in the batch reverses the scores (run with fixed_center_conv=True - with
-    the default False the reference itself makes tr/rot depend on the batch composition, DESIGN.md section 2)."""
+    the default False the reference itself makes tr/rot depend on the batch composition)."""
 import copy
 import math
 from functools import partial

@@ -87,7 +87,7 @@ def emulate(plan, ea, node, ns, tgt, src, x, vec, n_out, ew=None):
         mul_out, dout, rows = KINDS[kind]
         assert n_mma % 32 == 0 and nrow * mul_out <= n_mma <= mul_out * rows <= 192
         Wt = torch.zeros(E, mul_out * rows, dtype=torch.float64)         # columns beyond n_mma are never produced
-        Wt[:, :n_mma] = _mma(A, w2[t, :n_mma], H)                        # [E, N]: the TMEM accumulator tile
+        Wt[:, :n_mma] = _mma(A, w2[t, :n_mma], H)                        # [E, N]: the accumulator tile
         sh_off = (flags >> 8) & 0xff
         yb = torch.zeros(E, 5, dtype=torch.float64)
         for j in range(5):
@@ -140,7 +140,7 @@ def test_fused_plan_emulation_matches_oracle_layer(li):
 
 
 def test_fused_plan_tile_flags_and_limits():
-    """Tile table invariants the kernel relies on: N a multiple of 16 and <= 192 (two 8-row halves for a CTA pair), flag 1 on
+    """Tile table invariants the kernel relies on: N a multiple of 16 and <= 192 (the kernel's MMA width), flag 1 on
     the first / flag 2 on the last tile of every output irrep, flag 4 exactly where the path changes, tiles of one output
     irrep contiguous."""
     ns, nv = 48, 10

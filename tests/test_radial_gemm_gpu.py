@@ -1,4 +1,4 @@
-"""GPU: tcgen05 split-bf16 radial GEMM (csrc/radial_gemm.cu) vs an fp32 reference of the same Linear.
+"""GPU: wgmma split-bf16 radial GEMM (csrc/radial_gemm.cu) vs an fp32 reference of the same Linear.
 Tolerance: the 3-term bf16 split keeps ~16 mantissa bits per operand -> 3e-5 of the output's max magnitude."""
 import pytest
 import torch

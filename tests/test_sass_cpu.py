@@ -1,7 +1,8 @@
 """CPU: static check of the built library's machine code (cuobjdump -sass, tools/sass_histogram.py) - the hot kernels are written
-for Blackwell's tensor cores and copy engines, not recompiled legacy paths: tcgen05 MMAs (UTCHMMA, the 2-CTA form in the pair
-kernel), tensor-memory loads (LDTM), bulk copies (UBLKCP), multicast commits, no mma.sync (HMMA) anywhere; and the fused
-kernel's MMA issue block holds all eight MMAs of a staged k-block in one straight-line run (the v3 issue loop)."""
+for Hopper's tensor cores and copy engines, not recompiled legacy paths: warpgroup MMAs (HGMMA), bulk copies (UBLKCP), mbarrier
+operations, no mma.sync (HMMA) anywhere; and the fused kernel's issue block of one staged k-block holds exactly its eight
+bf16 MMAs, separated only by uniform predicate / descriptor moves, the skip of an empty slot and the register fence before
+each MMA - no wgmma wait, barrier or memory access inside the block."""
 import os
 import shutil
 import sys
@@ -25,17 +26,14 @@ def test_no_legacy_tensor_core_instructions(table):
     assert table and all(c['HMMA'] == 0 for c, _, _ in table.values())
 
 
-def test_fused_kernel_is_tcgen05_native(table):
-    pair = next(v for k, v in table.items() if 'fused_conv_kernel<2, 0>' in k)
-    single = next(v for k, v in table.items() if 'fused_conv_kernel<1, 0>' in k)
-    for counts, block, var in (pair, single):
-        assert counts['UTCHMMA'] >= 8 and counts['LDTM'] > 0 and counts['UBLKCP'] > 0 and counts['SYNCS'] > 0 and counts['REDG'] > 0
-        assert block == 8, block                      # one issue block per staged k-block
-    assert 'UTCHMMA.2CTA' in pair[2] and 'UTCBAR.2CTA.MULTICAST' in pair[2]
+def test_fused_kernel_is_wgmma_native(table):
+    counts, block, var = next(v for k, v in table.items() if 'fused_conv_kernel' in k)
+    assert counts['HGMMA'] >= 8 and counts['UBLKCP'] > 0 and counts['SYNCS'] > 0 and counts['REDG'] > 0
+    assert block == 8, block                          # the eight MMA slots of one staged k-block, nothing more
 
 
 def test_streaming_and_gemm_kernels_use_bulk_copies(table):
     tp = next(v for k, v in table.items() if 'tpconv_accumulate_kernel' in k)
-    assert tp[0]['UBLKCP'] > 0 and tp[0]['REDG'] > 0 and tp[0]['UTCHMMA'] == 0      # HBM-bound: no tensor cores by design
+    assert tp[0]['UBLKCP'] > 0 and tp[0]['REDG'] > 0 and tp[0]['HGMMA'] == 0        # HBM-bound: no tensor cores by design
     gemm = [v for k, v in table.items() if 'radial_gemm_kernel' in k]
-    assert gemm and all(c['UTCHMMA'] > 0 and c['LDTM'] > 0 for c, _, _ in gemm)
+    assert gemm and all(c['HGMMA'] > 0 and c['UBLKCP'] > 0 for c, _, _ in gemm)

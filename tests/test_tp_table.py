@@ -97,7 +97,7 @@ def test_c_abi_library_exports_every_declared_symbol(built_lib):
     assert sorted(_lib.SIGNATURES) == declared
     for name in declared:
         assert getattr(built_lib, name) is not None
-    assert b'sm_100a' in built_lib.ddb200_version()
+    assert b'sm_90a' in built_lib.ddb200_version()
 
 
 def test_product_refuses_cpu_tensors():

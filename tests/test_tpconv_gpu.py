@@ -42,7 +42,7 @@ def test_small_config(built_lib):
 
 @pytest.mark.parametrize("stage", [0, 1, 2, 3])
 def test_fully_fused_conv_matches_oracle(built_lib, stage):
-    """csrc/fused_conv.cu (radial MLP on tcgen05 + contraction out of TMEM + scatter, one kernel) vs the oracle layer.
+    """csrc/fused_conv.cu (radial MLP on wgmma + contraction from the on-chip accumulator tile + scatter, one kernel) vs the oracle layer.
     Tolerance 1e-4: two chained split-bf16 GEMMs feed the contraction."""
     from diffdock_b200 import fused
     assert fused.ENABLED

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of the fully fused convolution kernel alone (csrc/fused_conv.cu) on receptor-like edges of the full-width
-156 -> 156 layer: bf16 tcgen05 TFLOP/s issued, and - with DDB200_FUSED_DEBUG=1 - the clock breakdown of its warp roles.
-    python tools/bench_fused.py [--edges 400000] [--layer 3]        DDB200_FUSED_CTA_PAIR=0|1 selects the kernel variant"""
+156 -> 156 layer: bf16 wgmma TFLOP/s issued, and - with DDB200_FUSED_DEBUG=1 - the clocks per edge tile.
+    python tools/bench_fused.py [--edges 400000] [--layer 3]"""
 import argparse
 import ctypes as C
 import json
@@ -11,10 +11,6 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-
-NAMES = {0: 'mma_role', 1: 'mma_wait_acc_free', 2: 'mma_wait_B', 3: 'mma_wait_A2', 5: 'prod_wait_stage_free', 6: 'relay_wait_full', 7: 'relay_arrive',
-         8: 'cons_tile_loop', 9: 'cons_wait_hidden', 10: 'a0_build', 16: 'cons_M_build', 17: 'cons_body_kind0', 18: 'cons_body_other', 19: 'n_kind0', 20: 'n_other',
-         21: 'cons_flush', 22: 'cons_z', 23: 'cons_wait_acc', 24: 'cons_fma', 11: 'unit_total', 12: 'units'}
 
 def scan():
     """BASELINE config 4 for the kernel the model runs: receptor sizes 500-5000 x ligand sizes 20-80, 32 poses, full-width
@@ -59,7 +55,7 @@ def scan():
             ms = sorted(ts)[len(ts) // 2]
             nbytes = E * (4 * t.weight_numel + 16) + 4 * (N + 1) + 4 * N * t.d_in + 4 * N * t.d_out
             print(json.dumps({'n_res': n_r, 'n_lig': n_l, 'nodes': N, 'E': E, 'ms': round(ms, 3),
-                              'bf16_issued_TFLOPs': round(((E + 127) // 128) * plan.mma_flops_per_tile / ms / 1e9, 1),
+                              'bf16_issued_TFLOPs': round(((E + 63) // 64) * plan.mma_flops_per_tile / ms / 1e9, 1),
                               'algorithmic_TFLOPs': round(E * plan.alg_flops_per_edge / ms / 1e9, 1),
                               'equivalent_GBps': round(nbytes / ms / 1e6, 1), 'frac_of_hbm_peak': round(nbytes / ms / 1e6 / peak, 3)}),
                   flush=True)
@@ -113,15 +109,11 @@ if __name__ == '__main__':
         torch.cuda.synchronize()
         ts.append(e0.elapsed_time(e1))
     ms = sorted(ts)[2]
-    flops = ((E + 127) // 128) * plan.mma_flops_per_tile
-    r = {'E': E, 'tiles': plan.n_tiles, 'ms': round(ms, 3), 'bf16_issued_TFLOPs': round(flops / ms / 1e9, 1),
-         'pair': os.environ.get('DDB200_FUSED_CTA_PAIR', '1')}
+    flops = ((E + 63) // 64) * plan.mma_flops_per_tile
+    r = {'E': E, 'tiles': plan.n_tiles, 'ms': round(ms, 3), 'bf16_issued_TFLOPs': round(flops / ms / 1e9, 1)}
     if have_dbg and _lib.lib().ddb200_fused_debug_read(dbg) == 0:
-        pair = os.environ.get('DDB200_FUSED_CTA_PAIR', '1') != '0'
-        units = max(int(dbg[12]), 1)         # counted once per CTA: a pair unit counts twice
-        one_cta = {0, 1, 2, 3, 6, 7}         # counters only the leader (MMA role) or only the peer (relay) adds to
-        r['clk_per_cta_unit'] = {NAMES[i]: int(dbg[i]) * (2 if (pair and i in one_cta) else 1) // units for i in NAMES if i != 12}
-        r['units'] = units // 5
-        r['issue_clk_per_mma'] = round(dbg[13] / max(dbg[14], 1), 1)
+        units = max(int(dbg[12]), 1)
+        r['clk_per_edge_tile'] = int(dbg[11]) // units
+        r['edge_tiles'] = units // 5
         r['sm_clock_ghz_in_kernel'] = round(dbg[25] / max(dbg[26], 1), 3)     # clock64 ticks per globaltimer ns, CTA 0
     print(json.dumps(r), flush=True)

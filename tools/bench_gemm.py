@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Micro-benchmark of the tcgen05 split-bf16 radial GEMM alone: fp32-equivalent TFLOP/s (2*E*K*N), bf16 tensor TFLOP/s
+"""Micro-benchmark of the wgmma split-bf16 radial GEMM alone: fp32-equivalent TFLOP/s (2*E*K*N), bf16 tensor TFLOP/s
 actually issued (3x, K padded to 448) and output-write GB/s.   python tools/bench_gemm.py [--edges 200000]"""
 import argparse
 import json

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Reduce ncu CSV exports to the summaries kept under profiles/.
+"""Reduce ncu CSV exports to short per-kernel summaries (write them under build/profiles/, which git ignores).
     python tools/ncu_summarize.py raw <ncu --page raw --csv file> <out.csv> "<header comment>"
     python tools/ncu_summarize.py launches <ncu --metrics gpu__time_duration.sum --csv log> <out.csv> "<header comment>"
 """

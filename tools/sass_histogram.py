@@ -1,10 +1,11 @@
 #!/usr/bin/env python
 """Static instruction histogram of the built library (cuobjdump -sass): one row per kernel with the counts of the mnemonics
-that show what the code runs on - tcgen05 MMAs (UTCHMMA), their commits (UTCBAR), tensor-memory loads (LDTM), bulk / TMA copies
-(UBLKCP / UTMALDG), mbarrier operations (SYNCS), reductions to global memory (REDG) - and of the legacy ones it must not
-contain (HMMA = mma.sync).  Also the longest run of UTCHMMA separated only by uniform-datapath / move instructions: the size of
+that show what the code runs on - warpgroup MMAs (HGMMA), their register fences (WARPGROUP), bulk / TMA copies (UBLKCP /
+UTMALDG), mbarrier operations (SYNCS), reductions to global memory (REDG) - and of the legacy ones it must not contain (HMMA =
+mma.sync).  Also the longest run of bf16 HGMMA separated only by uniform-datapath / move instructions, the uniform skip
+of an empty slot and the register fence before each MMA (no wgmma wait, barrier or memory access in between): the size of
 the fused kernel's MMA issue block.
-    python tools/sass_histogram.py [lib.so] > profiles/<round>_sass_histogram.csv"""
+    mkdir -p build/profiles && python tools/sass_histogram.py [lib.so] > build/profiles/sass_histogram.csv"""
 import os
 import re
 import subprocess
@@ -12,11 +13,14 @@ import sys
 from collections import Counter, OrderedDict
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-COLS = ['UTCHMMA', 'UTCBAR', 'LDTM', 'STTM', 'UBLKCP', 'UTMALDG', 'SYNCS', 'ELECT', 'REDG', 'ATOMG', 'HMMA', 'FFMA', 'LDS', 'STS',
+COLS = ['HGMMA', 'WARPGROUP', 'UBLKCP', 'UTMALDG', 'SYNCS', 'ELECT', 'REDG', 'ATOMG', 'HMMA', 'FFMA', 'LDS', 'STS',
         'LDG', 'STG', 'SHFL', 'MUFU', 'UCGABAR', 'BAR']
-VARIANTS = ('UTCHMMA', 'UTCBAR', 'UBLKCP', 'LDTM', 'REDG')
-# instructions allowed between two MMAs of one issue block: predicate / uniform moves, register->uniform moves, adds
-GLUE = ('UMOV', 'R2UR', 'UISETP', 'IMAD', 'IADD3', 'NOP', 'UIADD3', 'LOP3', 'SHF', 'ISETP', 'P2R', 'MOV')
+VARIANTS = ('HGMMA', 'WARPGROUP', 'UBLKCP', 'REDG')
+# instructions allowed between two MMAs of one issue block: predicate / uniform moves, register->uniform moves, adds, the
+# uniform skip of an empty slot and the warpgroup register fence (WARPGROUP.ARRIVE) before each MMA.  Anything else - the
+# wgmma wait (WARPGROUP.DEPBAR), a barrier, a memory access - ends the block.
+GLUE = ('UMOV', 'R2UR', 'UISETP', 'IMAD', 'IADD3', 'NOP', 'UIADD3', 'LOP3', 'SHF', 'ISETP', 'P2R', 'MOV', 'PLOP3', 'BRA',
+        'VOTEU', 'WARPGROUP.ARRIVE')
 
 
 def kernels(lib):
@@ -28,7 +32,7 @@ def kernels(lib):
             cur = m.group(1)
             body[cur] = []
             continue
-        m = re.match(r'\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)', line)
+        m = re.match(r'\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Za-z0-9_.]*)', line)
         if m and cur is not None:
             body[cur].append(m.group(1))
     return body
@@ -47,10 +51,10 @@ def longest_mma_run(ops):
     best = run = 0
     for op in ops:
         base = op.split('.')[0]
-        if base == 'UTCHMMA':
+        if base == 'HGMMA' and '.BF16' in op:        # the project's MMAs (the compiler also emits an empty F16 HGMMA)
             run += 1
             best = max(best, run)
-        elif base not in GLUE:
+        elif base not in GLUE and op not in GLUE:
             run = 0
     return best
 
@@ -67,7 +71,7 @@ def rows(lib):
 if __name__ == '__main__':
     lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, 'diffdock_b200', 'libdiffdock_b200.so')
     print('# cuobjdump -sass diffdock_b200/libdiffdock_b200.so, instruction counts per kernel (static code, not executed counts);'
-          ' mma_block = longest run of UTCHMMA with only move / uniform glue in between')
+          ' mma_block = longest run of HGMMA with only move / uniform glue in between')
     print('kernel,instructions,' + ','.join(COLS) + ',mma_block,variants')
     for name, n, counts, block, var in sorted(rows(lib), key=lambda r: -r[1]):
         print(f'"{name}",{n},' + ','.join(map(str, counts)) + f',{block},"{var}"')
