@@ -101,6 +101,7 @@ struct FusedParams {
   const int* tgt; const int* src;                    // scatter target / gathered node of every edge
   const int* perm;                                   // optional: row of ea / vec / ew that belongs to edge e
   const float* ea_add; const int* ea_add_idx;        // optional: ea row += ea_add[ea_add_idx[e], :ne]
+  int a0_vec;                                        // A0' rows gathered with 16-byte loads (decided by the host)
   float vec_sign;
   const __nv_bfloat16* w1img; int K1, K1p, n_kb1, H, Hp, n_kb;
   const __nv_bfloat16* w2img;                        // [n_tiles][n_kb][256][64]
@@ -352,7 +353,7 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
       const long long e0 = mt * BM;
       const int Kin = p.K1, Kp = p.K1p;
       if (tid < BM) put_a_tail(sA, tid, Kin, Kp);
-      if (((p.ne | p.ns) & 7) == 0 && ((p.ld_ea | p.ld_node) & 3) == 0) {
+      if (p.a0_vec) {
         // vector path: four threads per edge row, each converting a contiguous quarter of the row's 8-column groups (<= 5
         // groups = 10 independent 16-byte loads).  The row's indices (attribute row, per-graph term, both end points) are
         // loaded once per thread, then ALL data loads of the thread are issued - including the per-graph term's - then the
@@ -606,6 +607,11 @@ extern "C" int ddb200_fused_conv(const ddb200_fused_args* a, void* stream) {
   FusedParams p = {};
   p.ea = a->edge_attr; p.ld_ea = a->ld_ea; p.ne = a->ne; p.node = a->node; p.ld_node = a->ld_node; p.ns = a->ns;
   p.tgt = a->tgt; p.src = a->src; p.perm = a->edge_perm; p.ea_add = a->ea_add; p.ea_add_idx = a->ea_add_idx;
+  // 16-byte loads of whole 8-column groups: every row that is read (edge_attr, ea_add, both node sections) must start on a
+  // 16-byte boundary, so the base pointers as well as the widths and row strides are checked
+  const auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  p.a0_vec = ((a->ne | a->ns) & 7) == 0 && ((a->ld_ea | (a->ns ? a->ld_node : 0)) & 3) == 0 && al16(a->edge_attr) &&
+             (a->ns == 0 || al16(a->node)) && (a->ea_add == nullptr || al16(a->ea_add));
   p.vec_sign = a->vec_sign == 0.f ? 1.f : a->vec_sign;
   p.w1img = reinterpret_cast<const __nv_bfloat16*>(a->w1_images); p.K1 = K1; p.K1p = K1p; p.n_kb1 = n_kb1;
   p.H = H; p.Hp = Hp; p.n_kb = n_kb;

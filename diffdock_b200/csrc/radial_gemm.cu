@@ -208,14 +208,17 @@ static int launch_radial(GemmParams& p, void* stream) {
   const int n_kb_max = p.n_kb > p.n_kb1 ? p.n_kb : p.n_kb1;
   const size_t smem = (size_t)n_kb_max * A_KB_BYTES + STAGES * B_STAGE_BYTES + 2 * STAGES * sizeof(uint64_t) + 1024;
   { const char* ns = getenv("DDB200_GEMM_NOSTORE"); p.debug_nostore = (ns && ns[0] == '1') ? 1 : 0; }
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t err = cudaFuncSetAttribute(radial_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (err != cudaSuccess) return (int)err;
-    attr_done = true;
-  }
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
+  // the opt-in to > 48 KB of dynamic shared memory is a per-device attribute: record it per device
+  constexpr int MAX_DEVICES = 64;
+  static bool attr_done[MAX_DEVICES] = {};
+  if (dev < 0 || dev >= MAX_DEVICES) return DDB200_EINVAL;
+  if (!attr_done[dev]) {
+    cudaError_t err = cudaFuncSetAttribute(radial_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (err != cudaSuccess) return (int)err;
+    attr_done[dev] = true;
+  }
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long n_mtiles = (p.n_edges + BM - 1) / BM;
   const unsigned grid = (unsigned)(n_mtiles < sms ? n_mtiles : sms);

@@ -213,6 +213,10 @@ int ddb200_radial_mlp(const float* edge_attr, int64_t ld_ea, int ne, const float
  * 16-column-aligned sections, N tiles = whole rows of one path block, dense Clebsch-Gordan tables [path][3][3][5] padded to
  * 48 floats).  Supported shapes: (mul_out, 2l_out+1) in {(48,1),(10,3),(16,1),(4,3)}, l_in <= 1, spherical harmonics from
  * edge vectors (sh_lmax <= 2), ne + 2 ns <= 144, hidden <= 144.
+ * Any base pointer and row stride is accepted.  The rows of a are read with 16-byte loads when ne % 8 == 0, ns % 8 == 0,
+ * ld_ea % 4 == 0, edge_attr 16-byte aligned, and (ns > 0) ld_node % 4 == 0 and node 16-byte aligned, and (ea_add given)
+ * ea_add 16-byte aligned; otherwise element by element.  x is read with 8-byte loads when x_pairs_ok, ld_x is even and x
+ * is 8-byte aligned; otherwise element by element.
  * Replaces: models/tensor_layers.py:139-144 / :204-221 including fc_layer(edge_attr) and the edge_attr_ assembly of
  * models/cg_model.py:342-349.  Follow with ddb200_tpconv_finalize.
  * ------------------------------------------------------------------------------------------------------------- */

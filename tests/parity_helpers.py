@@ -32,6 +32,97 @@ def rel_err(a, b):
     return float((a - b).abs().max() / b.abs().max().clamp_min(1e-30))
 
 
+# Cases of the fused convolution shared by the plan emulation (CPU) and the kernel tests (GPU).
+# Consumer kinds: (ns, nv) = (48, 10) has the (48, 1) / (10, 3) kinds, (16, 4) the (16, 1) / (4, 3) kinds; every stage of the
+# irreps sequence, with spherical harmonics up to l = 2, up to l = 1, and the closed-form l <= 1 product ('faster').
+KIND_GRID = [((ns, nv), stage, lmax, faster) for ns, nv in ((48, 10), (16, 4)) for stage in range(4)
+             for lmax, faster in ((2, False), (1, False), (1, True))]
+# (ne, ns, H) of the radial MLP: production shapes, then the element-wise A0 path (ne, ns not multiples of 8; neither
+# K1 = 30 nor H a multiple of 16), K1 > H, K1 < H and H < 64
+SHAPE_GRID = [(48, 48, 144), (16, 16, 48), (144, 0, 144), (48, 0, 48),
+              (20, 5, 100), (48, 48, 48), (16, 16, 144), (48, 0, 40)]
+
+
+def fused_table(ns, nv, stage, lmax, faster):
+    from diffdock_b200.tensor_layers import get_irrep_seq
+    from diffdock_b200.tp_table import build_table
+    seq = get_irrep_seq(ns, nv, False, False)
+    shs = '1x0e + 1x1o' if lmax == 1 else '1x0e + 1x1o + 1x2e'
+    return build_table(seq[min(stage, 3)], shs, seq[min(stage + 1, 3)], 'faster' if faster else 'fctp')
+
+
+def fused_weights(table, H, K1, gen):
+    """Radial MLP parameters (W1 [H, K1], b1, W2 [weight_numel, H] in reference row order, b2) at a trained model's scale."""
+    r = lambda *s: torch.randn(*s, generator=gen)
+    return r(H, K1) / K1 ** 0.5, 0.1 * r(H), r(table.weight_numel, H) / H ** 0.5, 0.1 * r(table.weight_numel)
+
+
+def irreps_str(irreps):
+    """[(mul, l, parity)] of a TpTable -> an irreps string the oracle parses."""
+    return ' + '.join(f'{m}x{l}{"e" if p == 1 else "o"}' for m, l, p in irreps)
+
+
+def fused_conv_reference(table, w1, b1, w2, b2, ea, node, ns, tgt, src, x, vec, n_out, ew=None, edge_perm=None,
+                         vec_sign=1.0, ea_add=None, ea_add_idx=None, device=None, chunk=2048):
+    """float64 restatement of the fused convolution of one edge group (include/diffdock_b200.h:ddb200_fused_conv):
+        r = edge_perm[e] (default e),  a = [ea[r, :ne] (+ ea_add[ea_add_idx[e]]) | node[tgt[e], :ns] | node[src[e], :ns]]
+        sum[tgt[e]] += TP(x[src[e]], Y(vec_sign * vec[r]), (relu(a W1^T + b1) W2^T + b2) * ew[r]),   cnt[tgt[e]] += 1
+    w2 / b2 are in the reference weight-row order.  Built only from plain torch and the oracle (spherical harmonics, the
+    FullyConnectedTensorProduct / FasterTensorProduct), evaluated chunk by chunk over the edges so that the per-edge weight
+    tensor never exists whole.  Returns (sum [n_out, d_out], cnt [n_out]) in float64 on ``device`` (default: ea's)."""
+    from oracle import e3nn_lite as o3
+    from oracle.tensor_layers import FasterTensorProduct
+    dev = torch.device(device) if device is not None else ea.device
+    ins, shs, outs = irreps_str(table.in_irreps), irreps_str(table.sh_irreps), irreps_str(table.out_irreps)
+    tp = FasterTensorProduct(ins, shs, outs) if table.kind == 'faster' else o3.FullyConnectedTensorProduct(ins, shs, outs)
+    tp = tp.to(dev)
+    assert tp.weight_numel == w2.shape[0] == table.weight_numel
+    d = lambda t: t.to(dev, torch.float64)
+    w1, b1, w2, b2, x = d(w1), d(b1), d(w2), d(b2), d(x)
+    ne = w1.shape[1] - 2 * ns
+    tgt, src = tgt.to(dev).long(), src.to(dev).long()
+    E = tgt.shape[0]
+    ea, vec = d(ea[:, :ne]), d(vec)
+    node = d(node[:, :ns]) if ns else None
+    ew = d(ew.reshape(-1)) if ew is not None else None
+    ea_add = d(ea_add) if ea_add is not None else None
+    out = torch.zeros(n_out, o3.Irreps(outs).dim, dtype=torch.float64, device=dev)
+    for c0 in range(0, E, chunk):
+        c1 = min(E, c0 + chunk)
+        r = edge_perm[c0:c1].to(dev).long() if edge_perm is not None else torch.arange(c0, c1, device=dev)
+        t, s = tgt[c0:c1], src[c0:c1]
+        a = ea[r]
+        if ea_add is not None:
+            a = a + ea_add[ea_add_idx[c0:c1].to(dev).long()]
+        if ns:
+            a = torch.cat([a, node[t], node[s]], 1)
+        w = torch.relu(a @ w1.T + b1) @ w2.T + b2
+        if ew is not None:
+            w = w * ew[r][:, None]
+        sh = o3.spherical_harmonics(o3.Irreps(shs), vec_sign * vec[r], normalize=True, normalization='component')
+        out.index_add_(0, t, tp(x[s], sh, w))
+    return out, torch.bincount(tgt, minlength=n_out).double()
+
+
+def block_errors(got, ref, out_irreps):
+    """Per output irrep block: max |got - ref| over the block / max |ref| over the block, the denominator floored at 1e-2 of
+    the global max |ref| (a near-zero block would otherwise turn rounding noise into a large ratio).  ``out_irreps`` is a
+    TpTable's [(mul, l, parity)].  Returns {'<mul>x<l><p>@<offset>': error}."""
+    got, ref = got.double(), ref.double().to(got.device)
+    floor = 1e-2 * float(ref.abs().max().clamp_min(1e-30))
+    errs, off = {}, 0
+    for m, l, p in out_irreps:
+        n = m * (2 * l + 1)
+        g, r = got[:, off:off + n], ref[:, off:off + n]
+        errs[f'{m}x{l}{"e" if p == 1 else "o"}@{off}'] = float((g - r).abs().max()) / max(float(r.abs().max()), floor)
+        off += n
+    return errs
+
+
+def max_block_err(got, ref, out_irreps):
+    return max(block_errors(got, ref, out_irreps).values())
+
+
 def layer_parity_case(seed=0, n_nodes=64, n_edges=700, ns=48, nv=10, lmax=2, stage=3, groups=1, faster=False,
                       device='cuda:0', reduce='mean', use_vec=True, edge_weight_tensor=False, out_nodes=None,
                       residual=True):

@@ -11,6 +11,8 @@ import torch
 from diffdock_b200 import fused
 from diffdock_b200.tensor_layers import get_irrep_seq
 from diffdock_b200.tp_table import build_table
+from tests.parity_helpers import (KIND_GRID, SHAPE_GRID, block_errors, fused_conv_reference, fused_table,
+                                  fused_weights)
 
 KINDS = {0: (48, 1, 4), 1: (10, 3, 16), 2: (16, 1, 8), 3: (4, 3, 16)}     # kind -> (mul_out, 2l_out+1, rows per tile)
 
@@ -137,6 +139,81 @@ def test_fused_plan_emulation_matches_oracle_layer(li):
     err = float((got - ref.double()).abs().max() / ref.abs().max())
     assert err < 3e-5, err          # split-bf16 x3: ~2^-16 relative per product, fp32-level after accumulation
     assert plan.n_tiles == len(plan.tiles) and plan.mma_flops_per_tile > 0
+
+
+@pytest.mark.parametrize("ns_nv,stage,lmax,faster", KIND_GRID)
+def test_emulation_consumer_kinds(ns_nv, stage, lmax, faster):
+    """Every consumer kind / stage / harmonics variant at the production (ne, ns, H): the emulated plan against the float64
+    reference, per output block."""
+    ns, nv = ns_nv
+    table = fused_table(ns, nv, stage, lmax, faster)
+    _emulation_case(table, ns, ns, 3 * ns, seed=200 + 10 * stage + lmax + 5 * faster + ns)
+
+
+@pytest.mark.parametrize("ne,ns,H", SHAPE_GRID)
+def test_emulation_radial_shapes(ne, ns, H):
+    _emulation_case(fused_table(48, 10, 3, 2, False), ne, ns, H, seed=ne + 3 * ns + H)
+
+
+def _emulation_case(table, ne, ns, H, seed, n_nodes=11, E=150):
+    assert fused.supported(table, H, ne + 2 * ns)
+    g = torch.Generator().manual_seed(seed)
+    w = fused_weights(table, H, ne + 2 * ns, g)
+    plan = fused.FusedPlan(table, *w)
+    x = torch.randn(n_nodes, table.d_in, generator=g)
+    node = torch.randn(n_nodes, max(ns, 1) + 2, generator=g)
+    tgt = torch.randint(0, n_nodes, (E,), generator=g)
+    src = torch.randint(0, n_nodes, (E,), generator=g)
+    ea, vec, ew = torch.randn(E, ne, generator=g), torch.randn(E, 3, generator=g), torch.rand(E, generator=g)
+    got = emulate(plan, ea, node, ns, tgt, src, x, vec, n_nodes, ew)
+    ref, _ = fused_conv_reference(table, *w, ea, node, ns, tgt, src, x, vec, n_nodes, ew=ew)
+    errs = block_errors(got, ref, table.out_irreps)
+    assert max(errs.values()) < 3e-5, errs         # the kernel's per-block tolerance; measured <= 1e-5
+
+
+@pytest.mark.parametrize("faster,ns,extras", [(False, 48, True), (False, 0, False), (True, 16, True), (True, 0, True)])
+def test_fp64_reference_matches_oracle_layer(faster, ns, extras):
+    """tests/parity_helpers.py:fused_conv_reference, followed by the mean, BatchNorm and residual, is the oracle
+    TensorProductConvLayer run in float64 (edge_perm / vec_sign / ea_add / edge_weight applied to the layer's inputs)."""
+    from oracle import e3nn_lite as o3
+    from oracle.tensor_layers import TensorProductConvLayer as OLayer
+    from tests.parity_helpers import irreps_str, rand_bn_
+    nv = 10 if ns != 16 else 4
+    table = fused_table(ns or 48, nv, 2, 1 if faster else 2, faster)
+    ins, shs, outs = irreps_str(table.in_irreps), irreps_str(table.sh_irreps), irreps_str(table.out_irreps)
+    ne, n_nodes, E = 24, 13, 200
+    n_out = n_nodes
+    K1 = ne + 2 * ns
+    torch.manual_seed(ns + faster)
+    layer = OLayer(ins, shs, outs, K1, hidden_features=40, faster=faster).double().eval()
+    g = torch.Generator().manual_seed(7 + ns)
+    rand_bn_(layer.batch_norm, g)
+    w = (layer.fc[0].weight, layer.fc[0].bias, layer.fc[-1].weight, layer.fc[-1].bias)
+    x = torch.randn(n_nodes, table.d_in, generator=g, dtype=torch.float64)
+    tgt = torch.randint(0, n_out - 4, (E,), generator=g)          # the last rows receive no edge: mean of nothing = 0
+    src = torch.randint(0, n_nodes, (E,), generator=g)
+    rows = 2 * E
+    ea, vec = torch.randn(rows, ne, generator=g, dtype=torch.float64), torch.randn(rows, 3, generator=g, dtype=torch.float64)
+    vec[3] = 0.0                                          # a zero-length edge vector
+    ew = torch.rand(rows, generator=g, dtype=torch.float64)
+    kw = {}
+    perm = torch.randperm(rows, generator=g)[:E] if extras else torch.arange(E)
+    if extras:
+        add, add_idx = torch.randn(3, ne, generator=g, dtype=torch.float64), torch.randint(0, 3, (E,), generator=g)
+        kw = dict(edge_perm=perm, vec_sign=-1.0, ea_add=add, ea_add_idx=add_idx)
+    sign = kw.get('vec_sign', 1.0)
+    a = ea[perm] + (add[add_idx] if extras else 0)
+    if ns:
+        a = torch.cat([a, x[tgt, :ns], x[src, :ns]], 1)
+    sh = o3.spherical_harmonics(o3.Irreps(shs), sign * vec[perm], normalize=True, normalization='component')
+    with torch.no_grad():
+        s, cnt = fused_conv_reference(table, *w, ea, x, ns, tgt, src, x, vec, n_out, ew=ew, **kw)
+        got = layer.batch_norm(s / cnt.clamp_min(torch.finfo(torch.float64).eps)[:, None])
+        got = got + torch.nn.functional.pad(x, (0, got.shape[1] - x.shape[1]))
+        ref = layer(x, torch.stack([tgt, src]), a, sh, out_nodes=n_out, edge_weight=ew[perm][:, None])
+    assert torch.equal(cnt, torch.bincount(tgt, minlength=n_out).double())
+    err = float((got - ref).abs().max() / ref.abs().max())
+    assert err < 1e-12, err
 
 
 def test_fused_plan_tile_flags_and_limits():
