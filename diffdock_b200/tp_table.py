@@ -64,6 +64,7 @@ class TpTable:
     sh_lmax: int                 # >= 0: SH evaluated in-kernel from the edge vector; -1: SH given per edge
     iblob: np.ndarray = field(default=None, repr=False)
     fblob: np.ndarray = field(default=None, repr=False)
+    fblob64: np.ndarray = field(default=None, repr=False)   # the same terms in float64 (fblob is their float32 rounding)
     stage_floats: int = 0
     n_chunks: int = 0
 
@@ -304,7 +305,8 @@ def _compile(t: TpTable, stage_floats: int):
     hdr[21] = o
     hdr[22:22 + len(lpr_list)] = lpr_list
     t.iblob = np.concatenate([hdr, s_paths, s_tiles, s_chunks, s_ment, s_ty, s_out]).astype(np.int32)
-    t.fblob = np.asarray(terms_v if terms_v else [0.0], dtype=np.float32)
+    t.fblob64 = np.asarray(terms_v if terms_v else [0.0], dtype=np.float64)
+    t.fblob = t.fblob64.astype(np.float32)
     t.stage_floats, t.n_chunks = stage_floats, len(chunks)
 
 
@@ -327,8 +329,9 @@ def spherical_harmonics_np(vec, lmax):
 
 def evaluate(t: TpTable, x, sh_or_vec, w_padded, edge_weight=None):
     """Numpy interpreter of the compiled blobs, lane by lane like the kernel: per-edge tensor-product messages
-    [E, D_out] (float64).  ``w_padded`` is in the kernel layout ([E, weight_numel_padded])."""
-    ib, fb = t.iblob, t.fblob.astype(np.float64)
+    [E, D_out] (float64).  ``w_padded`` is in the kernel layout ([E, weight_numel_padded]).  The Clebsch-Gordan terms are
+    read in float64 (``fblob64``), so the result is the table's arithmetic without the float32 rounding of the terms."""
+    ib, fb = t.iblob, np.asarray(t.fblob64 if t.fblob64 is not None else t.fblob, dtype=np.float64)
     (_, n_paths, n_tiles, n_chunks, n_ment, n_terms, d_in, d_sh, d_out, lmax, z_tot, m_tot, n_acc, wpad,
      _cap) = ib[:15]
     o_paths, o_tiles, o_chunks, o_ment, o_ty, o_out = ib[15:21]

@@ -1,4 +1,6 @@
 """Shared helpers of the parity tests: seeded random layers/graphs evaluated by the oracle (CPU) and the product (CUDA)."""
+import functools
+
 import torch
 
 
@@ -62,21 +64,68 @@ def irreps_str(irreps):
     return ' + '.join(f'{m}x{l}{"e" if p == 1 else "o"}' for m, l, p in irreps)
 
 
+def _reference_tp(table, dev):
+    """The oracle's tensor product of a TpTable (FullyConnectedTensorProduct or FasterTensorProduct) on ``dev``."""
+    from oracle import e3nn_lite as o3
+    from oracle.tensor_layers import FasterTensorProduct
+    ins, shs, outs = irreps_str(table.in_irreps), irreps_str(table.sh_irreps), irreps_str(table.out_irreps)
+    tp = FasterTensorProduct(ins, shs, outs) if table.kind == 'faster' else o3.FullyConnectedTensorProduct(ins, shs, outs)
+    assert tp.weight_numel == table.weight_numel
+    return tp.to(dev)
+
+
+def tp_scatter_reference(table, x, src, tgt, geo, w_ref, n_out, ew=None, device=None, chunk=2048, tp=None, out=None):
+    """float64 restatement of the streaming convolution (include/diffdock_b200.h:ddb200_tpconv_accumulate):
+        sum[tgt[e]] += TP(x[src[e]], Y_e, w_ref[e]) * ew[e],   cnt[tgt[e]] += 1
+    Y_e is the oracle's spherical harmonics of geo[e] (normalize=True, component normalisation) when the table evaluates
+    them from edge vectors (table.sh_lmax >= 0), otherwise geo[e] itself (given SH).  ``w_ref`` [E, weight_numel] is in the
+    reference's weight order.  Built only from plain torch and the oracle, evaluated chunk by chunk over the edges.
+    ``out``: a float64 [n_out, d_out] accumulator to add into.  Returns (sum, cnt) in float64 on ``device`` (default: x's)."""
+    from oracle import e3nn_lite as o3
+    dev = torch.device(device) if device is not None else x.device
+    tp = tp if tp is not None else _reference_tp(table, dev)
+    assert w_ref.shape[1] == table.weight_numel
+    x = x.to(dev, torch.float64)
+    tgt, src = tgt.to(dev).long(), src.to(dev).long()
+    E = tgt.shape[0]
+    shs = o3.Irreps(irreps_str(table.sh_irreps))
+    if out is None:
+        out = torch.zeros(n_out, table.d_out, dtype=torch.float64, device=dev)
+    for c0 in range(0, E, chunk):
+        c1 = min(E, c0 + chunk)
+        g = geo[c0:c1].to(dev, torch.float64)
+        sh = o3.spherical_harmonics(shs, g, normalize=True, normalization='component') if table.sh_lmax >= 0 else g
+        m = tp(x[src[c0:c1]], sh, w_ref[c0:c1].to(dev, torch.float64))
+        if ew is not None:
+            m = m * ew.reshape(-1)[c0:c1].to(dev, torch.float64)[:, None]
+        out.index_add_(0, tgt[c0:c1], m)
+    return out, torch.bincount(tgt, minlength=n_out).double()
+
+
+def kernel_weights(table, w_ref, stride=None, fill=float('nan')):
+    """Per-edge weight rows [E, stride] in the kernel's layout (table.w_perm) from reference-order rows [E, weight_numel].
+    Padding columns (w_perm == -1) and the columns past weight_numel_padded hold ``fill``: with NaN, a read of anything but
+    a weight shows up as NaN in the output."""
+    stride = stride or table.weight_numel_padded
+    assert stride >= table.weight_numel_padded
+    out = torch.full((w_ref.shape[0], stride), fill, dtype=w_ref.dtype, device=w_ref.device)
+    perm = torch.as_tensor(table.w_perm, device=w_ref.device)
+    cols = torch.nonzero(perm >= 0).reshape(-1)
+    out[:, cols] = w_ref[:, perm[cols]]
+    return out
+
+
 def fused_conv_reference(table, w1, b1, w2, b2, ea, node, ns, tgt, src, x, vec, n_out, ew=None, edge_perm=None,
                          vec_sign=1.0, ea_add=None, ea_add_idx=None, device=None, chunk=2048):
     """float64 restatement of the fused convolution of one edge group (include/diffdock_b200.h:ddb200_fused_conv):
         r = edge_perm[e] (default e),  a = [ea[r, :ne] (+ ea_add[ea_add_idx[e]]) | node[tgt[e], :ns] | node[src[e], :ns]]
         sum[tgt[e]] += TP(x[src[e]], Y(vec_sign * vec[r]), (relu(a W1^T + b1) W2^T + b2) * ew[r]),   cnt[tgt[e]] += 1
-    w2 / b2 are in the reference weight-row order.  Built only from plain torch and the oracle (spherical harmonics, the
-    FullyConnectedTensorProduct / FasterTensorProduct), evaluated chunk by chunk over the edges so that the per-edge weight
-    tensor never exists whole.  Returns (sum [n_out, d_out], cnt [n_out]) in float64 on ``device`` (default: ea's)."""
-    from oracle import e3nn_lite as o3
-    from oracle.tensor_layers import FasterTensorProduct
+    w2 / b2 are in the reference weight-row order.  The radial MLP is evaluated chunk by chunk over the edges, so that the
+    per-edge weight tensor never exists whole, and each chunk goes through tp_scatter_reference.  Returns
+    (sum [n_out, d_out], cnt [n_out]) in float64 on ``device`` (default: ea's)."""
     dev = torch.device(device) if device is not None else ea.device
-    ins, shs, outs = irreps_str(table.in_irreps), irreps_str(table.sh_irreps), irreps_str(table.out_irreps)
-    tp = FasterTensorProduct(ins, shs, outs) if table.kind == 'faster' else o3.FullyConnectedTensorProduct(ins, shs, outs)
-    tp = tp.to(dev)
-    assert tp.weight_numel == w2.shape[0] == table.weight_numel
+    tp = _reference_tp(table, dev)
+    assert w2.shape[0] == table.weight_numel
     d = lambda t: t.to(dev, torch.float64)
     w1, b1, w2, b2, x = d(w1), d(b1), d(w2), d(b2), d(x)
     ne = w1.shape[1] - 2 * ns
@@ -86,7 +135,7 @@ def fused_conv_reference(table, w1, b1, w2, b2, ea, node, ns, tgt, src, x, vec, 
     node = d(node[:, :ns]) if ns else None
     ew = d(ew.reshape(-1)) if ew is not None else None
     ea_add = d(ea_add) if ea_add is not None else None
-    out = torch.zeros(n_out, o3.Irreps(outs).dim, dtype=torch.float64, device=dev)
+    out = torch.zeros(n_out, table.d_out, dtype=torch.float64, device=dev)
     for c0 in range(0, E, chunk):
         c1 = min(E, c0 + chunk)
         r = edge_perm[c0:c1].to(dev).long() if edge_perm is not None else torch.arange(c0, c1, device=dev)
@@ -97,11 +146,52 @@ def fused_conv_reference(table, w1, b1, w2, b2, ea, node, ns, tgt, src, x, vec, 
         if ns:
             a = torch.cat([a, node[t], node[s]], 1)
         w = torch.relu(a @ w1.T + b1) @ w2.T + b2
-        if ew is not None:
-            w = w * ew[r][:, None]
-        sh = o3.spherical_harmonics(o3.Irreps(shs), vec_sign * vec[r], normalize=True, normalization='component')
-        out.index_add_(0, t, tp(x[s], sh, w))
+        tp_scatter_reference(table, x, s, t, vec_sign * vec[r], w, n_out, ew=ew[r] if ew is not None else None,
+                             device=dev, chunk=c1 - c0, tp=tp, out=out)
     return out, torch.bincount(tgt, minlength=n_out).double()
+
+
+def tp_table_grid():
+    """{name: TpTable} of the streaming kernel's table features (tile kinds, z kinds, column tiles, remainder rows, TMA
+    chunking, padding, given SH, D_in > 256), built with tp_table.build_table:
+      final / final_odd    the score model's final_conv (seq[3] -> 2x1o + 2x1e, lmax 2; -> 1x1o + 1x1e, lmax 1)
+      tor / tor_odd        tor_bond_conv with given SH (FullTensorProduct(sh, 2e): 45 / 20 columns)
+      ladder_*             every stage of the irreps ladder at four (ns, nv), fctp lmax 2 / lmax 1 / faster
+      second_*             second-order representations (generic tile kind, 2l+1 = 5, the default z kind)
+      wide                 D_in = 512, a 160x0e output split over two column tiles, three lanes-per-row values
+      small_stages         seq[3] -> seq[3] with 100-float TMA chunks: many chunks, pieces split with remainder rows"""
+    return _tp_table_grid()
+
+
+@functools.lru_cache(maxsize=None)
+def _tp_table_grid():
+    from diffdock_b200.irreps import irreps_str as ir_str
+    from diffdock_b200.tensor_layers import get_irrep_seq
+    from diffdock_b200.tp_table import build_table, full_tensor_product
+    sh1, sh2 = '1x0e+1x1o', '1x0e+1x1o+1x2e'
+    seq = get_irrep_seq(48, 10, False, False)
+    g = {'final': build_table(seq[3], sh2, '2x1o + 2x1e'),
+         'final_odd': build_table(seq[3], sh1, '1x1o + 1x1e'),
+         'tor': build_table(seq[3], ir_str(full_tensor_product(sh2, '1x2e')[1]), '48x0o + 48x0e', sh_from_vector=False),
+         'tor_odd': build_table(seq[3], ir_str(full_tensor_product(sh1, '1x2e')[1]), '48x0o', sh_from_vector=False)}
+    for ns, nv in ((48, 10), (16, 4), (6, 3), (24, 6)):
+        s = get_irrep_seq(ns, nv, False, False)
+        for stage in range(4):
+            for name, shs, kind in (('l2', sh2, 'fctp'), ('l1', sh1, 'fctp'), ('faster', sh1, 'faster')):
+                g[f'ladder_{ns}_{nv}_s{stage}_{name}'] = build_table(s[stage], shs, s[min(stage + 1, 3)], kind)
+    for ns, nv, red in ((48, 10, False), (5, 3, True)):
+        s = get_irrep_seq(ns, nv, True, red)
+        g[f'second_{ns}_{nv}'] = build_table(s[3], sh2, s[3])
+    g['wide'] = build_table('96x0e + 20x1o + 20x2e + 20x1e + 20x2o + 96x0o', sh2, '160x0e + 8x1o')
+    g['small_stages'] = build_table(seq[3], sh2, seq[3], stage_floats=100)
+    return g
+
+
+def table_sections(table):
+    """(paths [n, 8], tiles [n, 16], chunks [n, 4], ment [n, 3]) of a compiled table's int blob."""
+    ib = table.iblob
+    sec = lambda i, n, w: ib[ib[15 + i]:ib[15 + i] + w * n].reshape(-1, w)
+    return sec(0, ib[1], 8), sec(1, ib[2], 16), sec(2, ib[3], 4), sec(3, ib[4], 3)
 
 
 def block_errors(got, ref, out_irreps):

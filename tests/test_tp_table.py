@@ -11,6 +11,7 @@ from diffdock_b200.irreps import real_cg
 from diffdock_b200.tp_table import build_table, evaluate, full_tensor_product
 from oracle import e3nn_lite as o3
 from oracle.tensor_layers import FasterTensorProduct, get_irrep_seq
+from tests.parity_helpers import kernel_weights, table_sections, tp_scatter_reference, tp_table_grid
 
 
 def _case(ins, shs, outs, kind, lmax, given=False):
@@ -65,6 +66,47 @@ def test_heads_second_order_and_padding():
     f = o3.FullTensorProduct(o3.Irreps.spherical_harmonics(2), '2e')
     a, b = torch.randn(4, 9, dtype=torch.float64), torch.randn(4, 5, dtype=torch.float64)
     assert torch.allclose(f(a, b), torch.einsum('ea,eb,abc->ec', a, b, torch.from_numpy(T)), atol=1e-12)
+
+
+GRID = sorted(tp_table_grid())
+
+
+@pytest.mark.parametrize("name", GRID)
+def test_grid_tables_match_scatter_reference(name):
+    """The numpy interpreter of the compiled blobs, on kernel-layout rows from kernel_weights (zero fill), scattered onto
+    targets with repeats, against the float64 reference of the whole accumulate step (tp_scatter_reference)."""
+    t = tp_table_grid()[name]
+    g = torch.Generator().manual_seed(GRID.index(name))
+    E, n_out = 3, 3
+    x = torch.randn(5, t.d_in, generator=g, dtype=torch.float64)
+    src, tgt = torch.tensor([4, 0, 4]), torch.tensor([2, 0, 2])
+    geo = torch.randn(E, 3 if t.sh_lmax >= 0 else t.d_sh, generator=g, dtype=torch.float64)
+    w = torch.randn(E, t.weight_numel, generator=g, dtype=torch.float64)
+    ew = torch.tensor([0.5, -1.25, 2.0], dtype=torch.float64)
+    ref, cnt = tp_scatter_reference(t, x, src, tgt, geo, w, n_out, ew=ew)
+    msg = evaluate(t, x[src].numpy(), geo.numpy(), kernel_weights(t, w, fill=0.0).numpy(), edge_weight=ew.numpy())
+    got = np.zeros((n_out, t.d_out))
+    np.add.at(got, tgt.numpy(), msg)
+    assert cnt.tolist() == [1.0, 0.0, 2.0]
+    assert np.abs(got - ref.numpy()).max() <= 1e-12 * np.abs(ref.numpy()).max()
+    assert not ref[1].any()
+
+
+def test_grid_reaches_every_table_feature():
+    """The grid above exercises every table feature the kernel branches on; narrowing it fails here."""
+    kinds, zkinds, col_tiles, rem_rows, max_chunks, padded, d_in = set(), set(), 1, False, 0, False, 0
+    for t in tp_table_grid().values():
+        paths, tiles, chunks, _ = table_sections(t)
+        kinds |= set(tiles[:, 11].tolist())
+        zkinds |= set(paths[:, 7].tolist())
+        rem_rows |= bool(np.any(tiles[:, 2] >> 16 > 0))
+        max_chunks = max(max_chunks, len(chunks))
+        padded |= t.weight_numel_padded > t.weight_numel
+        d_in = max(d_in, t.d_in)
+        # every column tile of an output irrep has its own accumulator rows: more of them than outputs = a split output
+        col_tiles = max(col_tiles, len(set(tiles[:, 9].tolist())) - len(t.out_irreps) + 1)
+    assert kinds >= {0, 1, 2, 3, 4} and zkinds >= {0, 1, 2, 3, 4}
+    assert col_tiles > 1 and rem_rows and max_chunks > 8 and padded and d_in > 256
 
 
 def test_tma_chunks_are_aligned_and_cover_the_row():

@@ -1,4 +1,7 @@
-"""GPU parity: fused tensor-product convolution (csrc/tpconv.cu through the C ABI) vs the CPU oracle layer.
+"""GPU parity: TensorProductConvLayer vs the CPU oracle layer, whole output against its max magnitude.
+Each case runs whichever kernel the layer picks: edge groups of 64 edges or more with edge vectors and a fused-kernel
+shape go to csrc/fused_conv.cu, the rest (given SH, small groups, other shapes) to csrc/tpconv.cu.  The kernels themselves
+are tested per output irrep block against float64 in tests/test_fused_conv_fp64_gpu.py and tests/test_tpconv_fp64_gpu.py.
 Tolerance: fp32 arithmetic with a different summation order -> 2e-5 relative to the output's max magnitude
 (north_star asks 1e-4 on scores)."""
 import pytest
