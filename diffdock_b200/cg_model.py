@@ -20,7 +20,8 @@ from torch import nn
 
 from . import ops
 from .irreps import irreps_str, sh_irreps
-from .layers import AtomEncoder, GaussianSmearing
+from .layers import (AtomEncoder, GaussianSmearing, _mlp, check_forward, cross_cutoff, cross_graph, edge_cutoff, edge_weight,
+                     ligand_graph)
 from .synthetic import LIG_FEATURE_DIMS as lig_feature_dims, REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims
 from .tensor_layers import TensorProductConvLayer, get_irrep_seq
 from .tp_table import full_tensor_product
@@ -31,8 +32,20 @@ SO3_MIN_EPS, SO3_MAX_EPS, SO3_N_EPS = 0.0005, 4, 2000
 TORUS_SIGMA_MIN, TORUS_SIGMA_MAX, TORUS_SIGMA_N = 3e-3, 2, 5000
 
 
-def _mlp(n_in, n_hidden, n_out, dropout):
-    return nn.Sequential(nn.Linear(n_in, n_hidden), nn.ReLU(), nn.Dropout(dropout), nn.Linear(n_hidden, n_out))
+def _i32(t):
+    return t.to(torch.int32).contiguous()
+
+
+def _flat(w):
+    """Per-edge weights as the flat vector the kernels take; None for the scalar weight 1."""
+    return w.reshape(-1).contiguous() if torch.is_tensor(w) else None
+
+
+def _rr_joint(c, n_lig):
+    """(target, source) of the static receptor graph as int32 in the joint numbering [ligand | residues], once per batch."""
+    if n_lig not in c.setdefault('rr_tgt32', {}):
+        c['rr_tgt32'][n_lig] = (_i32(c['rr_tgt'] + n_lig), _i32(c['rr_src'] + n_lig))
+    return c['rr_tgt32'][n_lig]
 
 
 def _sh_l2(vec):
@@ -110,22 +123,14 @@ class CGModel(nn.Module):
         self.rec_distance_expansion = GaussianSmearing(0.0, rec_max_radius, D)
         self.cross_distance_expansion = GaussianSmearing(0.0, cross_max_distance, Dx)
 
-        seq = get_irrep_seq(ns, nv, use_second_order_repr, reduce_pseudoscalars)
-        faster = sh_lmax == 1 and not use_second_order_repr
-
-        def conv(i, groups):
-            return TensorProductConvLayer(in_irreps=seq[min(i, len(seq) - 1)], sh_irreps=self.sh_irreps,
-                                          out_irreps=seq[min(i + 1, len(seq) - 1)], n_edge_features=3 * ns,
-                                          hidden_features=3 * ns, residual=True, batch_norm=batch_norm, dropout=dropout,
-                                          faster=faster, tp_weights_layers=tp_weights_layers, edge_groups=groups)
-
-        self.rec_emb_layers = nn.ModuleList([conv(i, 1) for i in range(num_prot_emb_layers)])
+        self._irrep_seq = get_irrep_seq(ns, nv, use_second_order_repr, reduce_pseudoscalars)
+        self._conv_kw = dict(sh_irreps=self.sh_irreps, n_edge_features=3 * ns, hidden_features=3 * ns, residual=True,
+                             batch_norm=batch_norm, dropout=dropout, faster=sh_lmax == 1 and not use_second_order_repr,
+                             tp_weights_layers=tp_weights_layers)
+        self.rec_emb_layers = nn.ModuleList([self.conv(i, 1) for i in range(num_prot_emb_layers)])
         if embed_also_ligand:
-            self.lig_emb_layers = nn.ModuleList([conv(i, 1) for i in range(num_prot_emb_layers)])
-        last = num_prot_emb_layers + num_conv_layers - 1
-        self.conv_layers = nn.ModuleList([
-            conv(i, 1 if not differentiate_convolutions else (2 if i == last else 4))
-            for i in range(num_prot_emb_layers, num_prot_emb_layers + num_conv_layers)])
+            self.lig_emb_layers = nn.ModuleList([self.conv(i, 1) for i in range(num_prot_emb_layers)])
+        self.conv_layers = self._interaction_stack(4, 2)
 
         # translation / rotation head
         self.center_distance_expansion = GaussianSmearing(0.0, center_max_distance, D)
@@ -153,6 +158,19 @@ class CGModel(nn.Module):
         self.register_buffer('_torus_table', torch.from_numpy(z['torus_score_norm']).float(), persistent=False)
         self._sync_free = None
 
+    def conv(self, i, groups):
+        """Convolution ``i`` of the stack (protein embedding layers first) with ``groups`` radial MLPs."""
+        seq = self._irrep_seq
+        return TensorProductConvLayer(in_irreps=seq[min(i, len(seq) - 1)], out_irreps=seq[min(i + 1, len(seq) - 1)],
+                                      edge_groups=groups, **self._conv_kw)
+
+    def _interaction_stack(self, groups, last_groups):
+        """The interaction layers: ``groups`` radial MLPs per layer, ``last_groups`` in the last one, one without
+        differentiate_convolutions."""
+        P, L = self.num_prot_emb_layers, self.num_conv_layers
+        return nn.ModuleList([self.conv(i, 1 if not self.differentiate_convolutions else
+                                        (last_groups if i == P + L - 1 else groups)) for i in range(P, P + L)])
+
     # ---------------------------------------------------------------------------------------------------------
     def load_state_dict(self, state_dict, strict=True, **kw):
         """Accepts reference checkpoints: e3nn's TensorProduct modules register buffers (``*.tp.weight``,
@@ -170,10 +188,7 @@ class CGModel(nn.Module):
 
     # ---------------------------------------------------------------------------------------------------------
     def get_edge_weight(self, edge_vec, max_norm):
-        if self.smooth_edges:
-            nrm = torch.clip(edge_vec.norm(dim=-1) * np.pi / max_norm, max=np.pi)
-            return 0.5 * (torch.cos(nrm) + 1.0).unsqueeze(-1)
-        return 1.0
+        return edge_weight(edge_vec, max_norm, self.smooth_edges)
 
     def _so3_score_norm(self, eps):
         """utils/so3.py:89-93 evaluated on the device (fp32 index arithmetic, round-half-even like np.around)."""
@@ -203,25 +218,20 @@ class CGModel(nn.Module):
         if uniq is not None and uniq[2] == B and uniq[0] * B == rec.pos.shape[0] and uniq[1] * B == ei.shape[1]:
             # N poses of one complex (inference.py:236-239): embed the receptor ONCE and tile the result; the reference
             # recomputes the identical 1280-wide embedding for every pose of the batch (models/cg_model.py:272-295)
-            n1, e1 = uniq[0], uniq[1]
-            ei1 = ei[:, :e1]
-            vec1 = (rec.pos[ei1[1]] - rec.pos[ei1[0]]).float()
-            ea1 = self.rec_edge_embedding(self.rec_distance_expansion(vec1.norm(dim=-1)))
-            na1 = self.rec_node_embedding(rec.x[:n1])
-            ew1 = self.get_edge_weight(vec1, self.rec_max_radius)
-            for layer in self.rec_emb_layers:
-                ea_ = torch.cat([ea1, na1[ei1[0], :self.ns], na1[ei1[1], :self.ns]], -1)
-                na1 = layer(na1, ei1, ea_, None, edge_weight=ew1, edge_vec=vec1)
-            vec, rec_edge_attr, rec_node_attr = vec1.repeat(B, 1), ea1.repeat(B, 1), na1.repeat(B, 1)
-            ew = ew1.repeat(B, 1) if torch.is_tensor(ew1) else ew1
+            copies, n1, e1 = B, uniq[0], uniq[1]
         else:
-            vec = (rec.pos[ei[1]] - rec.pos[ei[0]]).float()
-            rec_edge_attr = self.rec_edge_embedding(self.rec_distance_expansion(vec.norm(dim=-1)))
-            rec_node_attr = self.rec_node_embedding(rec.x)
-            ew = self.get_edge_weight(vec, self.rec_max_radius)
-            for layer in self.rec_emb_layers:
-                ea_ = torch.cat([rec_edge_attr, rec_node_attr[ei[0], :self.ns], rec_node_attr[ei[1], :self.ns]], -1)
-                rec_node_attr = layer(rec_node_attr, ei, ea_, None, edge_weight=ew, edge_vec=vec)
+            copies, n1, e1 = 1, rec.pos.shape[0], ei.shape[1]
+        ei1 = ei[:, :e1]
+        vec = (rec.pos[ei1[1]] - rec.pos[ei1[0]]).float()
+        rec_edge_attr = self.rec_edge_embedding(self.rec_distance_expansion(vec.norm(dim=-1)))
+        rec_node_attr = self.rec_node_embedding(rec.x[:n1])
+        ew = self.get_edge_weight(vec, self.rec_max_radius)
+        for layer in self.rec_emb_layers:
+            ea_ = torch.cat([rec_edge_attr, rec_node_attr[ei1[0], :self.ns], rec_node_attr[ei1[1], :self.ns]], -1)
+            rec_node_attr = layer(rec_node_attr, ei1, ea_, None, edge_weight=ew, edge_vec=vec)
+        if copies > 1:
+            vec, rec_edge_attr, rec_node_attr = vec.repeat(B, 1), rec_edge_attr.repeat(B, 1), rec_node_attr.repeat(B, 1)
+            ew = ew.repeat(B, 1) if torch.is_tensor(ew) else ew
         rec.rec_node_attr, rr.rec_edge_attr, rr.edge_weight = rec_node_attr, rec_edge_attr, ew
         rr.edge_sh = None   # evaluated inside the convolution kernel from the edge vectors; kept for attribute parity
         # CSR order of the static receptor graph (target = edge_index[0])
@@ -247,7 +257,6 @@ class CGModel(nn.Module):
         the per-step edge buffers (upper bounds that hold for ANY pose), int32 views.  One host read per batch."""
         rec, lig, ll = data['receptor'], data['ligand'], data['ligand', 'ligand']
         B, dev = data.num_graphs, lig.pos.device
-        i32 = lambda t: t.to(torch.int32).contiguous()
         n_lig, n_rec = lig.batch.shape[0], rec.batch.shape[0]
         lig_cnt = (c['lig_ptr'][1:] - c['lig_ptr'][:-1])
         rec_cnt = (c['rec_ptr'][1:] - c['rec_ptr'][:-1])
@@ -255,16 +264,16 @@ class CGModel(nn.Module):
         c['lig_cnt_f'] = lig_cnt.float().unsqueeze(1)
         c['rec_max'] = int(host[1].max()) if B else 0
         c['cap_cross'] = int((host[0].long() * host[1].long()).sum())      # every ligand atom x every residue of its complex
-        c['lig_batch32'], c['rec_batch32'] = i32(lig.batch), i32(rec.batch)
-        c['rr_gid32'] = i32(c['rr_tgt_batch'])
+        c['lig_batch32'], c['rec_batch32'] = _i32(lig.batch), _i32(rec.batch)
+        c['rr_gid32'] = _i32(c['rr_tgt_batch'])
         # bond edges grouped by their convolution target (edge_index[0]), original order kept inside a group
         ei = ll.edge_index.long()
         order = torch.sort(ei[0], stable=True).indices
-        c['pre_col'] = i32(ei[1][order])
+        c['pre_col'] = _i32(ei[1][order])
         cnt = torch.bincount(ei[0], minlength=n_lig)[:n_lig] if ei.shape[1] else torch.zeros(n_lig, dtype=torch.long, device=dev)
         ptr = torch.zeros(n_lig + 1, dtype=torch.int32, device=dev)
         ptr[1:] = torch.cumsum(cnt, 0)
-        c['pre_ptr'], c['pre_cnt'] = ptr, i32(cnt)
+        c['pre_ptr'], c['pre_cnt'] = ptr, _i32(cnt)
         attr = ll.edge_attr.float()[order] if ei.shape[1] else torch.zeros((0, self.in_lig_edge_features), device=dev)
         c['pre_attr'] = torch.cat([attr, torch.zeros((1, attr.shape[1]), device=dev)], 0)     # row -1: "not a bond"
         # radius_graph(max_num_neighbors=32) = radius with cap 33 minus the self hit: an atom whose own index is not among its
@@ -272,41 +281,13 @@ class CGModel(nn.Module):
         c['cap_ll'] = int(ei.shape[1]) + 33 * n_lig
         c['bond_lig_batch'] = lig.batch[c['bonds'][0]] if c['n_bonds'] else None
         c['cap_tor'] = 32 * c['n_bonds']
-        c['bond_batch32'] = i32(c['bond_batch']) if c['n_bonds'] else None
+        c['bond_batch32'] = _i32(c['bond_batch']) if c['n_bonds'] else None
 
     def _ligand_graph(self, data, c):
-        """Bond edges + radius graph, sorted by convolution target (models/cg_model.py:467-497)."""
-        lig, ll = data['ligand'], data['ligand', 'ligand']
-        lig.node_sigma_emb = self.timestep_emb_func(lig.node_t['tr'])
-        pos = lig.pos.float()
-        centre, nbr, _ = ops.radius(pos, pos, c['lig_ptr'], lig.batch, r=self.lig_max_radius,
-                                    max_num_neighbors=33, exclude_self=True)      # radius_graph: cap 32 (+ self)
-        n_rad = nbr.shape[0]
-        row0 = torch.cat([ll.edge_index[0].long(), nbr.long()])      # target of the convolution
-        row1 = torch.cat([ll.edge_index[1].long(), centre.long()])   # gathered node
-        bond_attr = torch.cat([ll.edge_attr.float(),
-                               torch.zeros(n_rad, self.in_lig_edge_features, device=pos.device)], 0)
-        tgt, order = torch.sort(row0, stable=True)
-        src = row1[order]
-        vec = pos[src] - pos[tgt]
-        edge_attr = torch.cat([bond_attr[order], lig.node_sigma_emb[tgt], self.lig_distance_expansion(vec.norm(dim=-1))], 1)
-        node_attr = torch.cat([lig.x.float(), lig.node_sigma_emb], 1)
-        return node_attr, tgt, src, edge_attr, vec, self.get_edge_weight(vec, self.lig_max_radius)
-
-    def _cross_graph(self, data, c, cutoff):
-        """Ligand-receptor edges within the (per-complex) cutoff, sorted by ligand atom (models/cg_model.py:539-562)."""
-        lig, rec = data['ligand'], data['receptor']
-        lp, rp = lig.pos.float(), rec.pos.float()
-        if torch.is_tensor(cutoff):
-            li, ri, _ = ops.radius(rp, lp, c['rec_ptr'], lig.batch, r=1.0, r_per_graph=cutoff.reshape(-1),
-                                   max_num_neighbors=10000)
-        else:
-            li, ri, _ = ops.radius(rp, lp, c['rec_ptr'], lig.batch, r=float(cutoff), max_num_neighbors=10000)
-        li, ri = li.long(), ri.long()
-        vec = rp[ri] - lp[li]
-        edge_attr = torch.cat([lig.node_sigma_emb[li], self.cross_distance_expansion(vec.norm(dim=-1))], 1)
-        cutoff_d = cutoff.reshape(-1)[lig.batch[li]] if torch.is_tensor(cutoff) else cutoff
-        return li, ri, edge_attr, vec, self.get_edge_weight(vec, cutoff_d)
+        """Bond edges + radius graph, sorted stably by convolution target (models/cg_model.py:467-497)."""
+        tgt, src, attr, vec, ew, node = ligand_graph(self, data, c['lig_ptr'])
+        tgt, order = torch.sort(tgt, stable=True)
+        return node, tgt, src[order], attr[order], vec[order], ew[order] if torch.is_tensor(ew) else ew
 
     # ---------------------------------------------------------------------------------------------------------
     def sync_free_capable(self):
@@ -322,17 +303,28 @@ class CGModel(nn.Module):
 
     @torch.no_grad()
     def forward(self, data):
-        if self.training:
-            raise RuntimeError("diffdock_b200.CGModel is inference-only: call .eval()")
-        lig, rec = data['ligand'], data['receptor']
-        if not lig.pos.is_cuda:
-            raise RuntimeError("diffdock_b200.CGModel runs on CUDA tensors only (no CPU fallback): data.to('cuda')")
-        if self.no_aminoacid_identities:
-            rec.x = rec.x * 0
+        check_forward(self, data)
         c = self._static(data)
-        if self.sync_free_capable() and c['rec_max'] <= 10000:      # cap of the cross graph (models/cg_model.py:546) not binding
+        # the cap of the cross graphs (models/cg_model.py:546, models/aa_model.py:595,610) must not bind
+        if self.sync_free_capable() and max(c['rec_max'], c.get('atom_max', 0)) <= 10000:
             return self._forward_sync_free(data, c)
         return self._forward_host_sized(data, c)
+
+    def _interaction_layers(self, node, groups, n_last, merge=False, shared=None):
+        """The interaction layers over the joint graph; the last one only takes the first ``n_last`` groups, the edges that
+        end on ligand atoms (models/cg_model.py:347-349).  ``merge``: one radial MLP for all edge types runs them as a
+        single group (exactly-sized lists only).  ``shared = (accumulators, k)``: layer 0 starts from messages computed
+        elsewhere instead of running group ``k``."""
+        L = len(self.conv_layers)
+        for l, layer in enumerate(self.conv_layers):
+            use, init = (groups if l < L - 1 else groups[:n_last]), None
+            if l == 0 and shared is not None:
+                init, skip = shared
+                use = use[:skip] + [None] + use[skip + 1:]
+            if merge:
+                use = [tuple(torch.cat([g[k] for g in use]) if use[0][k] is not None else None for k in range(5))]
+            node = layer.forward_groups(node, use, gather_scalars=self.ns, init=init)
+        return node
 
     # ---------------------------------------------------------------------------------------------------------
     def _forward_sync_free(self, data, c):
@@ -342,91 +334,84 @@ class CGModel(nn.Module):
         take (capacity, device count).  Shapes are static for a given batch, so a reverse-diffusion step can be captured in
         a CUDA graph (diffdock_b200/sampling.py)."""
         lig, rec = data['ligand'], data['receptor']
-        ns, B = self.ns, data.num_graphs
-        dev = lig.pos.device
+        ns, n_lig = self.ns, lig.batch.shape[0]
         tr_sigma, rot_sigma, tor_sigma = self.t_to_sigma(*[data.complex_t[k] for k in ('tr', 'rot', 'tor')])
-        n_lig, n_rec = lig.batch.shape[0], rec.batch.shape[0]
-        pos, rpos = lig.pos.float().contiguous(), rec.pos.float().contiguous()
-        scan = lambda cnt: torch.cumsum(cnt, 0, dtype=torch.int32)
 
         # -- embeddings (models/cg_model.py:272-306) --------------------------------------------------------------
         sig = self.rec_sigma_embedding(self.timestep_emb_func(data.complex_t['tr'])).contiguous()      # [B, ns]
         rec_node = rec.rec_node_attr.clone()
         rec_node[:, :ns] += sig[rec.batch]
-        lig.node_sigma_emb = self.timestep_emb_func(lig.node_t['tr'])
-
-        # -- ligand graph: bonds + radius graph, CSR by target, built on the device (:467-497) -------------------------
-        cnt = ops.radius_count(pos, pos, c['lig_ptr'], c['lig_batch32'], r=self.lig_max_radius, max_num_neighbors=33,
-                               exclude_self=True) + c['pre_cnt']
-        incl = scan(cnt)
-        ll_n = incl[-1:]
-        ll_tgt, ll_src, ll_vec, ll_eid, _ = ops.graph_fill(
-            pos, pos, c['lig_ptr'], c['lig_batch32'], (incl - cnt).contiguous(), c['cap_ll'], r=self.lig_max_radius,
-            max_num_neighbors=33, exclude_self=True, pre_ptr=c['pre_ptr'], pre_col=c['pre_col'], want_eid=True, fill_row=0)
-        tgt_l = ll_tgt.long()
-        ll_attr = torch.cat([c['pre_attr'][ll_eid.long()], lig.node_sigma_emb[tgt_l],
-                             self.lig_distance_expansion(ll_vec.norm(dim=-1))], 1)
-        ll_ea = self.lig_edge_embedding(ll_attr)
-        ll_ew = self.get_edge_weight(ll_vec, self.lig_max_radius)
-        lig_node = self.lig_node_embedding(torch.cat([lig.x.float(), lig.node_sigma_emb], 1))
-        ewt = lambda w: w.reshape(-1).contiguous() if torch.is_tensor(w) else None
-        g_ll = (ll_tgt, ll_src, ll_ea, ll_vec, ewt(ll_ew), dict(n_edges_dev=ll_n))
-        for layer in self.lig_emb_layers:
-            lig_node = layer.forward_groups(lig_node, [g_ll], gather_scalars=ns)
+        lig_node, g_ll = self._ligand_graph_sync_free(data, c)
 
         # -- cross graph, both directions (:321-327, :539-562) ------------------------------------------------------------
-        if self.dynamic_max_cross:
-            rpg, r_cross = (tr_sigma * 3 + 20).reshape(-1).float().contiguous(), 1.0
-        else:
-            rpg, r_cross = None, float(self.cross_max_distance)
-        cap = c['cap_cross']
-        cnt = ops.radius_count(rpos, pos, c['rec_ptr'], c['lig_batch32'], r=r_cross, r_per_graph=rpg, max_num_neighbors=10000)
-        incl = scan(cnt)
-        lr_n = incl[-1:]
-        slot = torch.empty((n_lig, max(c['rec_max'], 1)), dtype=torch.int32, device=dev)
-        # rows beyond the live count must be valid (zero) when library ops gather over the whole buffer: the smooth edge
-        # weight, or the embedding MLP when its shape is outside the edge-embedding kernel's templates
-        smooth = self.smooth_edges or not ((self.cross_distance_expansion.offset.shape[0], ns) in ops.EDGE_EMBED_SHAPES
-                                           and len(self.cross_edge_embedding) == 4)
-        lr_tgt, lr_src, lr_vec, _, _ = ops.graph_fill(
-            rpos, pos, c['rec_ptr'], c['lig_batch32'], (incl - cnt).contiguous(), cap, r=r_cross, r_per_graph=rpg,
-            max_num_neighbors=10000, slot_out=slot, slot_ld=slot.shape[1], col_offset=n_lig, fill_row=0 if smooth else None)
-        cnt_r = ops.radius_count(pos, rpos, c['lig_ptr'], c['rec_batch32'], r=r_cross, r_per_graph=rpg,
-                                 max_num_neighbors=1 << 30)
-        incl_r = scan(cnt_r)
-        rl_tgt, rl_src, _, _, rl_perm = ops.graph_fill(
-            pos, rpos, c['lig_ptr'], c['rec_batch32'], (incl_r - cnt_r).contiguous(), cap, r=r_cross, r_per_graph=rpg,
-            max_num_neighbors=1 << 30, want_vec=False, slot_in=slot, y_ptr=c['rec_ptr'], slot_ld=slot.shape[1],
-            want_perm=True, row_offset=n_lig)
-        lr_ea = self._cross_edge_embedding(lig.node_sigma_emb, lr_vec, lr_tgt, lr_n)
-        lr_ew = None
-        if self.smooth_edges:
-            cutoff_d = rpg[lig.batch[lr_tgt.long()]] if rpg is not None else r_cross
-            lr_ew = ewt(self.get_edge_weight(lr_vec, cutoff_d))
+        r, rpg = cross_cutoff(self, tr_sigma)
+        g_lr, g_rl = self._cross_graph_sync_free(data, c, rec.pos.float().contiguous(), c['rec_ptr'], c['rec_batch32'],
+                                                 c['rec_max'], c['cap_cross'], r, rpg, n_lig, self.cross_edge_embedding,
+                                                 self.cross_distance_expansion, vec_sign=-1.0)
 
         # -- joint graph: four edge groups (:329-338) ---------------------------------------------------------------
         node = torch.cat([lig_node, rec_node], 0)
-        rr_tgt32 = c.setdefault('rr_tgt32', {}).get(n_lig)
-        if rr_tgt32 is None:
-            i32 = lambda t: t.to(torch.int32).contiguous()
-            rr_tgt32 = c['rr_tgt32'][n_lig] = (i32(c['rr_tgt'] + n_lig), i32(c['rr_src'] + n_lig))
-        groups = [
-            g_ll,                                                                                         # lig <- lig
-            (lr_tgt, lr_src, lr_ea, lr_vec, lr_ew, dict(n_edges_dev=lr_n)),                               # lig <- rec
-            (rr_tgt32[0], rr_tgt32[1], c['rr_ea'], c['rr_vec'], ewt(c['rr_ew']),
-             dict(ea_add=sig, ea_add_idx=c['rr_gid32'])),                                                 # rec <- rec
-            (rl_tgt, rl_src, lr_ea, lr_vec, lr_ew, dict(n_edges_dev=lr_n, edge_perm=rl_perm, vec_sign=-1.0)),   # rec <- lig
-        ]
-        L = len(self.conv_layers)
-        shared = self._shared_receptor_messages(data, c, rec, rec_node, sig, n_lig) if L > 1 else None
-        for l, layer in enumerate(self.conv_layers):
-            use = groups if l < L - 1 else groups[:2]       # last layer: only edges that end on ligand atoms (:347-349)
-            if l == 0 and shared is not None:               # receptor <- receptor messages of layer 0: computed once per complex
-                node = layer.forward_groups(node, [use[0], use[1], None, use[3]], gather_scalars=ns, init=shared)
-            else:
-                node = layer.forward_groups(node, use, gather_scalars=ns)
-        lig_node = node[:n_lig]
-        return self._heads(data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_free=True)
+        rr_tgt32 = _rr_joint(c, n_lig)
+        groups = [g_ll,                                                                                   # lig <- lig
+                  g_lr,                                                                                   # lig <- rec
+                  (rr_tgt32[0], rr_tgt32[1], c['rr_ea'], c['rr_vec'], _flat(c['rr_ew']),
+                   dict(ea_add=sig, ea_add_idx=c['rr_gid32'])),                                           # rec <- rec
+                  g_rl]                                                                                   # rec <- lig, Y(-v)
+        shared = self._shared_receptor_messages(data, c, rec, rec_node, sig, n_lig) if len(self.conv_layers) > 1 else None
+        node = self._interaction_layers(node, groups, 2, shared=(shared, 2) if shared is not None else None)
+        return self._heads(data, c, node[:n_lig], tr_sigma, rot_sigma, tor_sigma, sync_free=True)
+
+    def _ligand_graph_sync_free(self, data, c):
+        """Bonds + radius graph, CSR by target, built on the device (models/cg_model.py:467-497), and the ligand embedding
+        layers over it: ``(ligand node features, edge group)``."""
+        lig = data['ligand']
+        pos = lig.pos.float().contiguous()
+        lig.node_sigma_emb = self.timestep_emb_func(lig.node_t['tr'])
+        cnt = ops.radius_count(pos, pos, c['lig_ptr'], c['lig_batch32'], r=self.lig_max_radius, max_num_neighbors=33,
+                               exclude_self=True) + c['pre_cnt']
+        incl = torch.cumsum(cnt, 0, dtype=torch.int32)
+        tgt, src, vec, eid, _ = ops.graph_fill(
+            pos, pos, c['lig_ptr'], c['lig_batch32'], (incl - cnt).contiguous(), c['cap_ll'], r=self.lig_max_radius,
+            max_num_neighbors=33, exclude_self=True, pre_ptr=c['pre_ptr'], pre_col=c['pre_col'], want_eid=True, fill_row=0)
+        attr = torch.cat([c['pre_attr'][eid.long()], lig.node_sigma_emb[tgt.long()],
+                          self.lig_distance_expansion(vec.norm(dim=-1))], 1)
+        g = (tgt, src, self.lig_edge_embedding(attr), vec, _flat(self.get_edge_weight(vec, self.lig_max_radius)),
+             dict(n_edges_dev=incl[-1:]))
+        node = self.lig_node_embedding(torch.cat([lig.x.float(), lig.node_sigma_emb], 1))
+        for layer in self.lig_emb_layers:
+            node = layer.forward_groups(node, [g], gather_scalars=self.ns)
+        return node, g
+
+    def _cross_graph_sync_free(self, data, c, xpos, x_ptr, x_batch32, x_max, cap, r, rpg, col_off, mlp, gs, vec_sign):
+        """Ligand <- x edges (x: residues or receptor atoms at ``xpos``, numbered from ``col_off`` in the joint graph) in a
+        capacity buffer, and the x <- ligand direction as a permutation of them with the edge vector times ``vec_sign``:
+        ``(forward group, reverse group)`` (models/cg_model.py:539-562)."""
+        lig = data['ligand']
+        pos = lig.pos.float().contiguous()
+        n_lig = pos.shape[0]
+        cnt = ops.radius_count(xpos, pos, x_ptr, c['lig_batch32'], r=r, r_per_graph=rpg, max_num_neighbors=10000)
+        incl = torch.cumsum(cnt, 0, dtype=torch.int32)
+        n_dev = incl[-1:]
+        slot = torch.empty((n_lig, max(x_max, 1)), dtype=torch.int32, device=pos.device)
+        # rows beyond the live count must be valid (zero) when library ops gather over the whole buffer: the smooth edge
+        # weight, or the embedding MLP when its shape is outside the edge-embedding kernel's templates
+        padded_valid = self.smooth_edges or not self._edge_embed_in_kernel(mlp, gs)
+        f_tgt, f_src, vec, _, _ = ops.graph_fill(
+            xpos, pos, x_ptr, c['lig_batch32'], (incl - cnt).contiguous(), cap, r=r, r_per_graph=rpg,
+            max_num_neighbors=10000, slot_out=slot, slot_ld=slot.shape[1], col_offset=col_off,
+            fill_row=0 if padded_valid else None)
+        cnt_r = ops.radius_count(pos, xpos, c['lig_ptr'], x_batch32, r=r, r_per_graph=rpg, max_num_neighbors=1 << 30)
+        incl_r = torch.cumsum(cnt_r, 0, dtype=torch.int32)
+        b_tgt, b_src, _, _, perm = ops.graph_fill(
+            pos, xpos, c['lig_ptr'], x_batch32, (incl_r - cnt_r).contiguous(), cap, r=r, r_per_graph=rpg,
+            max_num_neighbors=1 << 30, want_vec=False, slot_in=slot, y_ptr=x_ptr, slot_ld=slot.shape[1], want_perm=True,
+            row_offset=col_off)
+        ea = self._cross_edge_embedding(lig.node_sigma_emb, vec, f_tgt, n_dev, mlp, gs)
+        ew = None
+        if self.smooth_edges:
+            ew = _flat(self.get_edge_weight(vec, edge_cutoff(r, rpg, lig.batch, f_tgt.long())))
+        return ((f_tgt, f_src, ea, vec, ew, dict(n_edges_dev=n_dev)),
+                (b_tgt, b_src, ea, vec, ew, dict(n_edges_dev=n_dev, edge_perm=perm, vec_sign=vec_sign)))
 
     def _shared_receptor_messages(self, data, c, rec, rec_node, sig, n_lig):
         """Layer-0 receptor<-receptor messages when the batch holds B poses of ONE complex at ONE diffusion time: the residue
@@ -442,9 +427,8 @@ class CGModel(nn.Module):
             return None
         layer = self.conv_layers[0]
         if 'rr0' not in c:          # copy 0 of the CSR-sorted contact graph (targets of copy 0 sort first), local numbering
-            i32 = lambda t: t.to(torch.int32).contiguous()
-            c['rr0'] = (i32(c['rr_tgt'][:e1]), i32(c['rr_src'][:e1]), c['rr_ea'][:e1].contiguous(), c['rr_vec'][:e1].contiguous(),
-                        c['rr_ew'][:e1].reshape(-1).contiguous() if c['rr_ew'] is not None else None)
+            c['rr0'] = (_i32(c['rr_tgt'][:e1]), _i32(c['rr_src'][:e1]), c['rr_ea'][:e1].contiguous(),
+                        c['rr_vec'][:e1].contiguous(), _flat(c['rr_ew'][:e1]) if c['rr_ew'] is not None else None)
         t0, s0, ea0, vec0, ew0 = c['rr0']
         zero_idx = c.setdefault('rr0_zero', torch.zeros(e1, dtype=torch.int32, device=ea0.device))
         g0 = (t0, s0, ea0, vec0, ew0, dict(ea_add=sig[:1].contiguous(), ea_add_idx=zero_idx))
@@ -456,15 +440,15 @@ class CGModel(nn.Module):
         cnt_buf[n_lig:].view(B, n1).add_(cnt0.unsqueeze(0))
         return sum_buf, cnt_buf
 
-    def _cross_edge_embedding(self, node_sigma_emb, vec, row, n_dev, mlp=None, gs=None):
-        """cross_edge_embedding(cat[sigma_emb[lig], RBF(d)]) (models/cg_model.py:326,553-554): the sigma half of the first
-        Linear is applied per ligand NODE, the rest per edge in one kernel (ddb200_edge_embed).  ``mlp`` / ``gs``: another
-        embedding MLP / distance expansion of the same form (the all-atom model's ligand-residue and ligand-atom edges)."""
-        mlp = self.cross_edge_embedding if mlp is None else mlp
-        gs = self.cross_distance_expansion if gs is None else gs
+    def _edge_embed_in_kernel(self, mlp, gs):
+        return (gs.offset.shape[0], self.ns) in ops.EDGE_EMBED_SHAPES and len(mlp) == 4
+
+    def _cross_edge_embedding(self, node_sigma_emb, vec, row, n_dev, mlp, gs):
+        """``mlp(cat[sigma_emb[lig], gs(d)])`` (models/cg_model.py:326,553-554): the sigma half of the first Linear is
+        applied per ligand NODE, the rest per edge in one kernel (ddb200_edge_embed)."""
         l1, l2 = mlp[0], mlp[-1]
         S = node_sigma_emb.shape[1]
-        if (gs.offset.shape[0], self.ns) in ops.EDGE_EMBED_SHAPES and len(mlp) == 4:
+        if self._edge_embed_in_kernel(mlp, gs):
             u = torch.addmm(l1.bias, node_sigma_emb, l1.weight[:, :S].t()).contiguous()
             return ops.edge_embed(vec, row, u, l1.weight[:, S:].contiguous(), l2.weight.contiguous(), l2.bias.contiguous(),
                                   gs.offset.contiguous(), float(gs.coeff), n_dev)
@@ -475,8 +459,7 @@ class CGModel(nn.Module):
     def _forward_host_sized(self, data, c):
         """Forward with exactly-sized neighbour lists (one host read of each edge count): convolution shapes outside the
         fused kernel's templates, or more than 10000 residues per complex."""
-        lig, rec = data['ligand'], data['receptor']
-        ns, B = self.ns, data.num_graphs
+        rec, ns = data['receptor'], self.ns
         tr_sigma, rot_sigma, tor_sigma = self.t_to_sigma(*[data.complex_t[k] for k in ('tr', 'rot', 'tor')])
 
         # -- embeddings (models/cg_model.py:272-306) --------------------------------------------------------------
@@ -494,34 +477,24 @@ class CGModel(nn.Module):
             lig_node = layer(lig_node, ll_ei, ea_, None, edge_weight=ll_ew, edge_vec=ll_vec, assume_sorted=True)
 
         # -- cross graph (:321-327) ---------------------------------------------------------------------------------
-        cutoff = (tr_sigma * 3 + 20).unsqueeze(1) if self.dynamic_max_cross else self.cross_max_distance
-        li, ri, lr_ea, lr_vec, lr_ew = self._cross_graph(data, c, cutoff)
-        lr_ea = self.cross_edge_embedding(lr_ea)
+        r, rpg = cross_cutoff(self, tr_sigma)
+        li, ri, lr_ea, lr_vec, lr_ew = cross_graph(self, data, rec.pos.float(), c['rec_ptr'], r, rpg,
+                                                   self.cross_distance_expansion, self.cross_edge_embedding)
 
         # -- joint graph: four edge groups, each CSR-sorted by target (:329-338) ------------------------------------
         n_lig = lig_node.shape[0]
         node = torch.cat([lig_node, rec_node], 0)
         rl_tgt, rev = torch.sort(ri, stable=True)            # receptor <- ligand direction: same pairs, sorted by residue
-        i32 = lambda t: t.to(torch.int32).contiguous()
-        ewt = lambda w: w.reshape(-1).contiguous() if torch.is_tensor(w) else None
-        rr_tgt32 = c.setdefault('rr_tgt32', {}).get(n_lig)
-        if rr_tgt32 is None:      # static receptor graph: int32 indices in the joint numbering, once per batch
-            rr_tgt32 = c['rr_tgt32'][n_lig] = (i32(c['rr_tgt'] + n_lig), i32(c['rr_src'] + n_lig))
+        rr_tgt32 = _rr_joint(c, n_lig)
         groups = [   # (target, gathered node, edge attr, edge vector, edge weight): int32, CSR-sorted, built once per forward
-            (i32(ll_tgt), i32(ll_src), ll_ea, ll_vec.contiguous(), ewt(ll_ew)),                          # lig <- lig
-            (i32(li), i32(ri + n_lig), lr_ea, lr_vec.contiguous(), ewt(lr_ew)),                          # lig <- rec
-            (rr_tgt32[0], rr_tgt32[1], rr_ea, c['rr_vec'], ewt(c['rr_ew'])),                             # rec <- rec
-            (i32(rl_tgt + n_lig), i32(li[rev]), lr_ea[rev], (-lr_vec[rev]).contiguous(),
-             ewt(lr_ew[rev]) if torch.is_tensor(lr_ew) else None),                                       # rec <- lig, SH(-v)
+            (_i32(ll_tgt), _i32(ll_src), ll_ea, ll_vec.contiguous(), _flat(ll_ew)),                      # lig <- lig
+            (_i32(li), _i32(ri + n_lig), lr_ea, lr_vec.contiguous(), _flat(lr_ew)),                      # lig <- rec
+            (rr_tgt32[0], rr_tgt32[1], rr_ea, c['rr_vec'], _flat(c['rr_ew'])),                           # rec <- rec
+            (_i32(rl_tgt + n_lig), _i32(li[rev]), lr_ea[rev], (-lr_vec[rev]).contiguous(),
+             _flat(lr_ew[rev]) if torch.is_tensor(lr_ew) else None),                                     # rec <- lig, SH(-v)
         ]
-        L = len(self.conv_layers)
-        for l, layer in enumerate(self.conv_layers):
-            use = groups if l < L - 1 else groups[:2]       # last layer: only edges that end on ligand atoms (:347-349)
-            if not self.differentiate_convolutions:         # one radial MLP for all edge types: a single merged group
-                use = [tuple(torch.cat([g[k] for g in use]) if use[0][k] is not None else None for k in range(5))]
-            node = layer.forward_groups(node, use, gather_scalars=ns)
-        lig_node = node[:n_lig]
-        return self._heads(data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_free=False)
+        node = self._interaction_layers(node, groups, 2, merge=not self.differentiate_convolutions)
+        return self._heads(data, c, node[:n_lig], tr_sigma, rot_sigma, tor_sigma, sync_free=False)
 
     def _heads(self, data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_free):
         lig = data['ligand']

@@ -1,9 +1,87 @@
 """Embedding layers with the reference's parameter names (models/layers.py) - plain PyTorch modules on the device
-(small dense ops; the hot convolution lives in csrc/)."""
+(small dense ops; the hot convolution lives in csrc/) - and the graph plumbing the four models share."""
+import numpy as np
 import torch
 from torch import nn
 
+from . import ops
 from .tensor_layers import FCBlock  # noqa: F401  (re-export: the reference keeps FCBlock in models/layers.py)
+
+
+def _mlp(n_in, n_hidden, n_out, dropout):
+    return nn.Sequential(nn.Linear(n_in, n_hidden), nn.ReLU(), nn.Dropout(dropout), nn.Linear(n_hidden, n_out))
+
+
+def edge_weight(edge_vec, max_norm, smooth):
+    """Smooth cosine cut-off of the edges (models/cg_model.py:459); the scalar 1 when edges are not smoothed."""
+    if smooth:
+        nrm = torch.clip(edge_vec.norm(dim=-1) * np.pi / max_norm, max=np.pi)
+        return 0.5 * (torch.cos(nrm) + 1.0).unsqueeze(-1)
+    return 1.0
+
+
+def check_forward(model, data):
+    """What every forward checks first: inference mode and CUDA inputs; ``no_aminoacid_identities`` zeroes the residue
+    features in place as the reference does."""
+    name = type(model).__name__
+    if model.training:
+        raise RuntimeError(f"diffdock_b200.{name} is inference-only: call .eval()")
+    if not data['ligand'].pos.is_cuda:
+        raise RuntimeError(f"diffdock_b200.{name} runs on CUDA tensors only (no CPU fallback): data.to('cuda')")
+    if model.no_aminoacid_identities:
+        data['receptor'].x = data['receptor'].x * 0
+
+
+def cross_cutoff(model, tr_sigma):
+    """``(r, r_per_graph)`` of the ligand-receptor radius search (models/cg_model.py:321-327): 3 sigma_tr + 20 A per complex
+    with ``dynamic_max_cross``, else ``cross_max_distance``."""
+    if model.dynamic_max_cross:
+        return 1.0, (tr_sigma * 3 + 20).reshape(-1).float().contiguous()
+    return float(model.cross_max_distance), None
+
+
+def edge_cutoff(r, r_per_graph, batch, row):
+    """The cut-off of each edge for the smooth edge weight; ``batch[row]`` is the graph of each edge."""
+    return r_per_graph[batch[row]] if r_per_graph is not None else r
+
+
+def ligand_graph(model, data, lig_ptr):
+    """Bond edges + radius graph of the ligand (models/cg_model.py:467-497) in their original order: ``(target, source,
+    edge attribute input, vector source - target, edge weight, node input)``; sets ``node_sigma_emb`` on the ligand."""
+    lig, ll = data['ligand'], data['ligand', 'ligand']
+    lig.node_sigma_emb = model.timestep_emb_func(lig.node_t['tr'])
+    pos = lig.pos.float()
+    centre, nbr, _ = ops.radius(pos, pos, lig_ptr, lig.batch, r=model.lig_max_radius, max_num_neighbors=33,
+                                exclude_self=True)      # radius_graph: cap 32 (+ self)
+    tgt = torch.cat([ll.edge_index[0].long(), nbr.long()])
+    src = torch.cat([ll.edge_index[1].long(), centre.long()])
+    vec = pos[src] - pos[tgt]
+    bond_attr = torch.cat([ll.edge_attr.float(), pos.new_zeros(nbr.shape[0], model.in_lig_edge_features)], 0)
+    attr = torch.cat([bond_attr, lig.node_sigma_emb[tgt], model.lig_distance_expansion(vec.norm(dim=-1))], 1)
+    node = torch.cat([lig.x.float(), lig.node_sigma_emb], 1)
+    return tgt, src, attr, vec, model.get_edge_weight(vec, model.lig_max_radius), node
+
+
+def cross_graph(model, data, xpos, x_ptr, r, r_per_graph, expansion, mlp):
+    """Ligand <- x edges within the cut-off (x: residues or receptor atoms at ``xpos`` with segment pointers ``x_ptr``,
+    models/cg_model.py:539-562), grouped by ligand atom: ``(ligand index, x index, embedded edge attributes, vector x - ligand,
+    edge weight)``.  Needs ``node_sigma_emb`` on the ligand."""
+    lig = data['ligand']
+    lp = lig.pos.float()
+    li, xi, _ = ops.radius(xpos, lp, x_ptr, lig.batch, r=r, r_per_graph=r_per_graph, max_num_neighbors=10000)
+    li, xi = li.long(), xi.long()
+    vec = xpos[xi] - lp[li]
+    ea = mlp(torch.cat([lig.node_sigma_emb[li], expansion(vec.norm(dim=-1))], 1))
+    return li, xi, ea, vec, model.get_edge_weight(vec, edge_cutoff(r, r_per_graph, lig.batch, li))
+
+
+def confidence_head(model, data, lig_node):
+    """Mean of the ligand scalars per complex through ``confidence_predictor`` (models/old_cg_model.py:298-299)."""
+    ns, B, batch = model.ns, data.num_graphs, data['ligand'].batch
+    scal = torch.cat([lig_node[:, :ns], lig_node[:, -ns:]], 1) if model.num_conv_layers >= 3 else lig_node[:, :ns]
+    pooled = torch.zeros((B, scal.shape[1]), device=scal.device, dtype=scal.dtype).index_add_(0, batch, scal)
+    pooled = pooled / torch.bincount(batch, minlength=B).clamp(min=1).unsqueeze(1)
+    return model.confidence_predictor(pooled).squeeze(dim=-1)
 
 
 class GaussianSmearing(nn.Module):

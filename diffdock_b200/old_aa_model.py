@@ -15,21 +15,17 @@ CUDA only, inference only.  No CPU fallback.
 """
 from __future__ import annotations
 
-import numpy as np
 import torch
 import torch.nn.functional as F
 from torch import nn
 
 from . import ops
 from .irreps import irreps_str, sh_irreps
-from .layers import GaussianSmearing, OldAtomEncoder
+from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_forward, confidence_head, cross_cutoff, cross_graph,
+                     edge_weight, ligand_graph)
 from .synthetic import (LIG_FEATURE_DIMS as lig_feature_dims, REC_ATOM_FEATURE_DIMS as rec_atom_feature_dims,
                         REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims)
 from .tensor_layers import OldTensorProductConvLayer
-
-
-def _mlp(n_in, n_hidden, n_out, dropout):
-    return nn.Sequential(nn.Linear(n_in, n_hidden), nn.ReLU(), nn.Dropout(dropout), nn.Linear(n_hidden, n_out))
 
 
 class AAOldModel(nn.Module):
@@ -98,10 +94,7 @@ class AAOldModel(nn.Module):
         return super().load_state_dict(sd, strict=strict, **kw)
 
     def get_edge_weight(self, edge_vec, max_norm):                      # models/old_aa_model.py:352-356
-        if self.smooth_edges:
-            nn_ = torch.clip(edge_vec.norm(dim=-1) * np.pi / max_norm, max=np.pi)
-            return 0.5 * (torch.cos(nn_) + 1.0).unsqueeze(-1)
-        return 1.0
+        return edge_weight(edge_vec, max_norm, self.smooth_edges)
 
     def _static_graph(self, data, nt, pos, edge_embedding, node_embedding, expansion, max_r):
         """Receptor-residue / receptor-atom graph on precomputed edges (:400-445); row 0 = target, row 1 = gathered node."""
@@ -115,31 +108,16 @@ class AAOldModel(nn.Module):
 
     @torch.no_grad()
     def forward(self, data):                                            # models/old_aa_model.py:202-286
-        if self.training:
-            raise RuntimeError("diffdock_b200.AAOldModel is inference-only: call .eval()")
+        check_forward(self, data)
         lig_s, rec_s, atom_s = data['ligand'], data['receptor'], data['atom']
-        if not lig_s.pos.is_cuda:
-            raise RuntimeError("diffdock_b200.AAOldModel runs on CUDA tensors only (no CPU fallback): data.to('cuda')")
-        if self.no_aminoacid_identities:
-            rec_s.x = rec_s.x * 0
         B, ns, L, C = data.num_graphs, self.ns, self.num_conv_layers, self.conv_layers
         tr_sigma = data.complex_t['tr']                                 # confidence mode: times are used as they are (:209)
-        lp, rp, ap = lig_s.pos.float(), rec_s.pos.float(), atom_s.pos.float()
-        lig_ptr = ops.segment_ptr(lig_s.batch, B)
-        rec_ptr, atom_ptr = ops.segment_ptr(rec_s.batch, B), ops.segment_ptr(atom_s.batch, B)
+        rp, ap = rec_s.pos.float(), atom_s.pos.float()
 
         # ligand graph (:358-398): bonds + radius graph
-        lig_s.node_sigma_emb = self.timestep_emb_func(lig_s.node_t['tr'])
-        ll = data['ligand', 'ligand']
-        centre, nbr, _ = ops.radius(lp, lp, lig_ptr, lig_s.batch, r=self.lig_max_radius, max_num_neighbors=33,
-                                    exclude_self=True)                  # radius_graph: cap 32 (+ self)
-        lig_ei = torch.stack([torch.cat([ll.edge_index[0].long(), nbr.long()]),
-                              torch.cat([ll.edge_index[1].long(), centre.long()])])
-        lig_vec = lp[lig_ei[1]] - lp[lig_ei[0]]
-        lig_ea = torch.cat([torch.cat([ll.edge_attr.float(), lp.new_zeros(nbr.shape[0], self.in_lig_edge_features)], 0),
-                            lig_s.node_sigma_emb[lig_ei[0]], self.lig_distance_expansion(lig_vec.norm(dim=-1))], 1)
-        lig_w = self.get_edge_weight(lig_vec, self.lig_max_radius)
-        lig = self.lig_node_embedding(torch.cat([lig_s.x.float(), lig_s.node_sigma_emb], 1))
+        tgt, src, lig_ea, lig_vec, lig_w, lig_x = ligand_graph(self, data, ops.segment_ptr(lig_s.batch, B))
+        lig_ei = torch.stack([tgt, src])
+        lig = self.lig_node_embedding(lig_x)
         lig_ea = self.lig_edge_embedding(lig_ea)
 
         rec, rec_ei, rec_ea, rec_vec, rec_w = self._static_graph(data, 'receptor', rp, self.rec_edge_embedding,
@@ -150,23 +128,13 @@ class AAOldModel(nn.Module):
                                                               self.lig_max_radius)
 
         # cross graphs (:447-491): ligand-residue (cut-off per complex), ligand-atom (lig_max_radius), atom-residue (given)
-        if self.dynamic_max_cross:
-            cutoff = (tr_sigma * 3 + 20).reshape(-1)
-            li, ri, _ = ops.radius(rp, lp, rec_ptr, lig_s.batch, r=1.0, r_per_graph=cutoff, max_num_neighbors=10000)
-        else:
-            cutoff = self.cross_max_distance
-            li, ri, _ = ops.radius(rp, lp, rec_ptr, lig_s.batch, r=float(cutoff), max_num_neighbors=10000)
-        lr = torch.stack([li.long(), ri.long()])
-        lr_vec = rp[lr[1]] - lp[lr[0]]
-        lr_ea = self.lr_edge_embedding(torch.cat([lig_s.node_sigma_emb[lr[0]],
-                                                  self.cross_distance_expansion(lr_vec.norm(dim=-1))], 1))
-        lr_w = self.get_edge_weight(lr_vec, cutoff[lig_s.batch[lr[0]]] if torch.is_tensor(cutoff) else cutoff)
-        la_l, la_a, _ = ops.radius(ap, lp, atom_ptr, lig_s.batch, r=float(self.lig_max_radius), max_num_neighbors=10000)
-        la = torch.stack([la_l.long(), la_a.long()])
-        la_vec = ap[la[1]] - lp[la[0]]
-        la_ea = self.la_edge_embedding(torch.cat([lig_s.node_sigma_emb[la[0]],
-                                                  self.cross_distance_expansion(la_vec.norm(dim=-1))], 1))
-        la_w = self.get_edge_weight(la_vec, self.lig_max_radius)
+        r, rpg = cross_cutoff(self, tr_sigma)
+        li, ri, lr_ea, lr_vec, lr_w = cross_graph(self, data, rp, ops.segment_ptr(rec_s.batch, B), r, rpg,
+                                                  self.cross_distance_expansion, self.lr_edge_embedding)
+        la_l, la_a, la_ea, la_vec, la_w = cross_graph(self, data, ap, ops.segment_ptr(atom_s.batch, B),
+                                                      float(self.lig_max_radius), None, self.cross_distance_expansion,
+                                                      self.la_edge_embedding)
+        lr, la = torch.stack([li, ri]), torch.stack([la_l, la_a])
         ar = data['atom', 'receptor'].edge_index.long()
         ar_vec = rp[ar[1]] - ap[ar[0]]
         ar_ea = self.ar_edge_embedding(torch.cat([atom_s.node_sigma_emb[ar[0]],
@@ -197,7 +165,4 @@ class AAOldModel(nn.Module):
             if l != L - 1:
                 atom = F.pad(atom, (0, at_up.shape[-1] - atom.shape[-1])) + at_up + al_up + ar_up
                 rec = F.pad(rec, (0, rec_up.shape[-1] - rec.shape[-1])) + rec_up + ra_up + rl_up
-        scal = torch.cat([lig[:, :ns], lig[:, -ns:]], 1) if L >= 3 else lig[:, :ns]
-        pooled = torch.zeros((B, scal.shape[1]), device=scal.device, dtype=scal.dtype).index_add_(0, lig_s.batch, scal)
-        pooled = pooled / torch.bincount(lig_s.batch, minlength=B).clamp(min=1).unsqueeze(1)
-        return self.confidence_predictor(pooled).squeeze(dim=-1)
+        return confidence_head(self, data, lig)

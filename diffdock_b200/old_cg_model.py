@@ -12,20 +12,16 @@ CUDA only, inference only.  No CPU fallback.
 """
 from __future__ import annotations
 
-import numpy as np
 import torch
 import torch.nn.functional as F
 from torch import nn
 
 from . import ops
 from .irreps import irreps_str, sh_irreps
-from .layers import GaussianSmearing, OldAtomEncoder
+from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_forward, confidence_head, cross_cutoff, cross_graph,
+                     edge_weight, ligand_graph)
 from .synthetic import LIG_FEATURE_DIMS as lig_feature_dims, REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims
 from .tensor_layers import OldTensorProductConvLayer
-
-
-def _mlp(n_in, n_hidden, n_out, dropout):
-    return nn.Sequential(nn.Linear(n_in, n_hidden), nn.ReLU(), nn.Dropout(dropout), nn.Linear(n_hidden, n_out))
 
 
 class CGOldModel(nn.Module):
@@ -93,37 +89,20 @@ class CGOldModel(nn.Module):
         return super().load_state_dict(sd, strict=strict, **kw)
 
     def get_edge_weight(self, edge_vec, max_norm):                      # models/old_cg_model.py:353-359
-        if self.smooth_edges:
-            nn_ = torch.clip(edge_vec.norm(dim=-1) * np.pi / max_norm, max=np.pi)
-            return 0.5 * (torch.cos(nn_) + 1.0).unsqueeze(-1)
-        return 1.0
+        return edge_weight(edge_vec, max_norm, self.smooth_edges)
 
     @torch.no_grad()
     def forward(self, data):                                            # models/old_cg_model.py:203-301
-        if self.training:
-            raise RuntimeError("diffdock_b200.CGOldModel is inference-only: call .eval()")
+        check_forward(self, data)
         lig, rec = data['ligand'], data['receptor']
-        if not lig.pos.is_cuda:
-            raise RuntimeError("diffdock_b200.CGOldModel runs on CUDA tensors only (no CPU fallback): data.to('cuda')")
-        if self.no_aminoacid_identities:
-            rec.x = rec.x * 0
         B, ns = data.num_graphs, self.ns
         tr_sigma = data.complex_t['tr']                                 # confidence mode: times are used as they are
-        lp, rp = lig.pos.float(), rec.pos.float()
-        lig_ptr, rec_ptr = ops.segment_ptr(lig.batch, B), ops.segment_ptr(rec.batch, B)
+        rp = rec.pos.float()
 
         # ligand graph (:361-391): bonds + radius graph; row 0 = convolution target, row 1 = gathered node
-        lig.node_sigma_emb = self.timestep_emb_func(lig.node_t['tr'])
-        ll = data['ligand', 'ligand']
-        centre, nbr, _ = ops.radius(lp, lp, lig_ptr, lig.batch, r=self.lig_max_radius, max_num_neighbors=33,
-                                    exclude_self=True)                  # radius_graph: cap 32 (+ self)
-        lig_ei = torch.stack([torch.cat([ll.edge_index[0].long(), nbr.long()]),
-                              torch.cat([ll.edge_index[1].long(), centre.long()])])
-        lig_vec = lp[lig_ei[1]] - lp[lig_ei[0]]
-        lig_ea = torch.cat([torch.cat([ll.edge_attr.float(), lp.new_zeros(nbr.shape[0], self.in_lig_edge_features)], 0),
-                            lig.node_sigma_emb[lig_ei[0]], self.lig_distance_expansion(lig_vec.norm(dim=-1))], 1)
-        lig_ew = self.get_edge_weight(lig_vec, self.lig_max_radius)
-        lig_node = self.lig_node_embedding(torch.cat([lig.x.float(), lig.node_sigma_emb], 1))
+        tgt, src, lig_ea, lig_vec, lig_ew, lig_x = ligand_graph(self, data, ops.segment_ptr(lig.batch, B))
+        lig_ei = torch.stack([tgt, src])
+        lig_node = self.lig_node_embedding(lig_x)
         lig_ea = self.lig_edge_embedding(lig_ea)
 
         # receptor graph (:393-414)
@@ -136,18 +115,10 @@ class CGOldModel(nn.Module):
         rec_node = self.rec_node_embedding(torch.cat([rec.x.float(), rec.node_sigma_emb], 1))
 
         # cross graph (:439-461): row 0 = ligand atom, row 1 = receptor residue, vector receptor - ligand
-        if self.dynamic_max_cross:
-            cutoff = (tr_sigma * 3 + 20).reshape(-1)
-            li, ri, _ = ops.radius(rp, lp, rec_ptr, lig.batch, r=1.0, r_per_graph=cutoff, max_num_neighbors=10000)
-        else:
-            cutoff = self.cross_max_distance
-            li, ri, _ = ops.radius(rp, lp, rec_ptr, lig.batch, r=float(cutoff), max_num_neighbors=10000)
-        li, ri = li.long(), ri.long()
+        r, rpg = cross_cutoff(self, tr_sigma)
+        li, ri, lr_ea, lr_vec, lr_ew = cross_graph(self, data, rp, ops.segment_ptr(rec.batch, B), r, rpg,
+                                                   self.cross_distance_expansion, self.cross_edge_embedding)
         lr_ei, rl_ei = torch.stack([li, ri]), torch.stack([ri, li])
-        lr_vec = rp[ri] - lp[li]
-        lr_ea = self.cross_edge_embedding(torch.cat([lig.node_sigma_emb[li],
-                                                     self.cross_distance_expansion(lr_vec.norm(dim=-1))], 1))
-        lr_ew = self.get_edge_weight(lr_vec, cutoff[lig.batch[li]] if torch.is_tensor(cutoff) else cutoff)
 
         L = len(self.lig_conv_layers)
         for l in range(L):
@@ -166,7 +137,4 @@ class CGOldModel(nn.Module):
             lig_node = F.pad(lig_node, (0, lig_intra.shape[-1] - lig_node.shape[-1])) + lig_intra + lig_inter
             if l != L - 1:
                 rec_node = F.pad(rec_node, (0, rec_intra.shape[-1] - rec_node.shape[-1])) + rec_intra + rec_inter
-        scal = torch.cat([lig_node[:, :ns], lig_node[:, -ns:]], 1) if self.num_conv_layers >= 3 else lig_node[:, :ns]
-        pooled = torch.zeros((B, scal.shape[1]), device=scal.device, dtype=scal.dtype).index_add_(0, lig.batch, scal)
-        pooled = pooled / torch.bincount(lig.batch, minlength=B).clamp(min=1).unsqueeze(1)
-        return self.confidence_predictor(pooled).squeeze(dim=-1)
+        return confidence_head(self, data, lig_node)
