@@ -79,6 +79,11 @@ class AAModel(CGModel):
         form concatenates edge lists, which needs their sizes on the host)."""
         return self.differentiate_convolutions and super().sync_free_capable()
 
+    def sync_free_crop_capable(self):
+        """No per-step cropping on the sync-free path: the reference crops the receptor atoms too (utils/utils.py:388-413),
+        which the masked crop of CGModel does not cover; the sampler keeps the eager crop for this model."""
+        return False
+
     # ---------------------------------------------------------------------------------------------------------
     @staticmethod
     def _csr(tgt, src, n_rows, *payload):

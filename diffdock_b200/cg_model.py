@@ -225,6 +225,8 @@ class CGModel(nn.Module):
         vec = (rec.pos[ei1[1]] - rec.pos[ei1[0]]).float()
         rec_edge_attr = self.rec_edge_embedding(self.rec_distance_expansion(vec.norm(dim=-1)))
         rec_node_attr = self.rec_node_embedding(rec.x[:n1])
+        if self.rec_emb_layers:     # input of the embedding layers: a cropped step runs them over its own contact graph
+            c['rec_node_pre'] = rec_node_attr.repeat(copies, 1)
         ew = self.get_edge_weight(vec, self.rec_max_radius)
         for layer in self.rec_emb_layers:
             ea_ = torch.cat([rec_edge_attr, rec_node_attr[ei1[0], :self.ns], rec_node_attr[ei1[1], :self.ns]], -1)
@@ -301,6 +303,11 @@ class CGModel(nn.Module):
             self._sync_free = bool(ok)
         return self._sync_free
 
+    def sync_free_crop_capable(self):
+        """The sync-free forward can also crop the receptor per step (``data._crop``, set by the sampler's graphed step): the
+        receptor embedding layers then run on every step over the cropped contact graph, so they need the fused kernel too."""
+        return self.sync_free_capable() and all(layer.fused_capable(self.ns, self.ns) for layer in self.rec_emb_layers)
+
     @torch.no_grad()
     def forward(self, data):
         check_forward(self, data)
@@ -308,6 +315,9 @@ class CGModel(nn.Module):
         # the cap of the cross graphs (models/cg_model.py:546, models/aa_model.py:595,610) must not bind
         if self.sync_free_capable() and max(c['rec_max'], c.get('atom_max', 0)) <= 10000:
             return self._forward_sync_free(data, c)
+        if getattr(data, '_crop', None) is not None:
+            raise RuntimeError("per-step receptor cropping (data._crop) runs on the sync-free forward only, which this "
+                               "batch cannot take (more than 10000 residues in a complex)")
         return self._forward_host_sized(data, c)
 
     def _interaction_layers(self, node, groups, n_last, merge=False, shared=None):
@@ -339,27 +349,59 @@ class CGModel(nn.Module):
 
         # -- embeddings (models/cg_model.py:272-306) --------------------------------------------------------------
         sig = self.rec_sigma_embedding(self.timestep_emb_func(data.complex_t['tr'])).contiguous()      # [B, ns]
-        rec_node = rec.rec_node_attr.clone()
+        crop = getattr(data, '_crop', None)
+        if crop is None:
+            rec_node, rec_pos = rec.rec_node_attr.clone(), rec.pos.float().contiguous()
+            rr_tgt32 = _rr_joint(c, n_lig)
+            g_rr = (rr_tgt32[0], rr_tgt32[1], c['rr_ea'], c['rr_vec'], _flat(c['rr_ew']),
+                    dict(ea_add=sig, ea_add_idx=c['rr_gid32']))
+        else:
+            rec_node, rec_pos, g_rr = self._cropped_receptor(data, c, crop, sig, n_lig)
         rec_node[:, :ns] += sig[rec.batch]
         lig_node, g_ll = self._ligand_graph_sync_free(data, c)
 
         # -- cross graph, both directions (:321-327, :539-562) ------------------------------------------------------------
         r, rpg = cross_cutoff(self, tr_sigma)
-        g_lr, g_rl = self._cross_graph_sync_free(data, c, rec.pos.float().contiguous(), c['rec_ptr'], c['rec_batch32'],
+        g_lr, g_rl = self._cross_graph_sync_free(data, c, rec_pos, c['rec_ptr'], c['rec_batch32'],
                                                  c['rec_max'], c['cap_cross'], r, rpg, n_lig, self.cross_edge_embedding,
                                                  self.cross_distance_expansion, vec_sign=-1.0)
 
         # -- joint graph: four edge groups (:329-338) ---------------------------------------------------------------
         node = torch.cat([lig_node, rec_node], 0)
-        rr_tgt32 = _rr_joint(c, n_lig)
         groups = [g_ll,                                                                                   # lig <- lig
                   g_lr,                                                                                   # lig <- rec
-                  (rr_tgt32[0], rr_tgt32[1], c['rr_ea'], c['rr_vec'], _flat(c['rr_ew']),
-                   dict(ea_add=sig, ea_add_idx=c['rr_gid32'])),                                           # rec <- rec
+                  g_rr,                                                                                   # rec <- rec
                   g_rl]                                                                                   # rec <- lig, Y(-v)
-        shared = self._shared_receptor_messages(data, c, rec, rec_node, sig, n_lig) if len(self.conv_layers) > 1 else None
+        # the shared layer-0 messages assume every pose keeps every residue
+        shared = self._shared_receptor_messages(data, c, rec, rec_node, sig, n_lig) \
+            if len(self.conv_layers) > 1 and crop is None else None
         node = self._interaction_layers(node, groups, 2, shared=(shared, 2) if shared is not None else None)
         return self._heads(data, c, node[:n_lig], tr_sigma, rot_sigma, tor_sigma, sync_free=True)
+
+    def _cropped_receptor(self, data, c, crop, sig, n_lig):
+        """utils/sampling.py:104-109 in masked form: the residues farther than the step's cut-off from every ligand atom of
+        their complex keep their rows but lose every edge.  ``crop = (cutoff2_table, step_dev)``.  Returns the receptor node
+        features (the embedding layers rerun over the cropped contact graph, as the reference embeds its cropped batch),
+        the positions for the cross-graph search (+inf at dropped residues) and the rec <- rec edge group."""
+        if not self.sync_free_crop_capable():
+            raise RuntimeError("per-step receptor cropping needs every receptor embedding layer on the fused kernel "
+                               "(CGModel.sync_free_crop_capable)")
+        lig, rec = data['ligand'], data['receptor']
+        keep, rec_pos = ops.crop_flags(lig.pos.float().contiguous(), c['lig_ptr'], rec.pos.float().contiguous(),
+                                       c['rec_batch32'], crop[0], crop[1])
+        if 'rr_tgt32l' not in c:
+            c['rr_tgt32l'] = (_i32(c['rr_tgt']), _i32(c['rr_src']))
+        tgt, src, perm, gid, n_dev = ops.crop_select_edges(*c['rr_tgt32l'], keep, c['rr_gid32'], offset=n_lig)
+        ew = _flat(c['rr_ew'])
+        if len(self.rec_emb_layers):
+            node = c['rec_node_pre']
+            g = (tgt - n_lig, src - n_lig, c['rr_ea'], c['rr_vec'], ew, dict(n_edges_dev=n_dev, edge_perm=perm))
+            for layer in self.rec_emb_layers:
+                node = layer.forward_groups(node, [g], gather_scalars=self.ns)
+        else:
+            node = rec.rec_node_attr.clone()
+        g_rr = (tgt, src, c['rr_ea'], c['rr_vec'], ew, dict(n_edges_dev=n_dev, edge_perm=perm, ea_add=sig, ea_add_idx=gid))
+        return node, rec_pos, g_rr
 
     def _ligand_graph_sync_free(self, data, c):
         """Bonds + radius graph, CSR by target, built on the device (models/cg_model.py:467-497), and the ligand embedding

@@ -285,6 +285,51 @@ def pose_update_dev(pos, n_poses, bond_u, bond_v, mask_rotate_u8, tr_score, rot_
     return out
 
 
+def crop_flags(lig_pos, lig_ptr, rec_pos, rec_batch32, cutoff2_table, step_dev=None):
+    """Residues within the cut-off of some ligand atom of their complex (ddb200_crop_flags): ``(keep bool [n_rec], receptor
+    positions with +inf at dropped residues [n_rec, 3])``; the squared cut-off is row ``*step_dev`` of ``cutoff2_table``."""
+    _need_cuda(lig_pos, lig_ptr, rec_pos, rec_batch32, cutoff2_table)
+    for t in (lig_pos, rec_pos, cutoff2_table):
+        assert t.dtype == torch.float32 and t.is_contiguous()
+    assert lig_ptr.dtype == torch.int32 and rec_batch32.dtype == torch.int32
+    if step_dev is not None:
+        assert step_dev.dtype == torch.int32 and step_dev.is_cuda
+    n_rec = rec_pos.shape[0]
+    keep = torch.empty(n_rec, dtype=torch.bool, device=rec_pos.device)
+    masked = torch.empty_like(rec_pos)
+    rc = _lib.lib().ddb200_crop_flags(_ptr(lig_pos), _ptr(lig_ptr), _ptr(rec_pos), _ptr(rec_batch32), n_rec,
+                                      _ptr(cutoff2_table), _ptr(step_dev), _ptr(keep), _ptr(masked), _stream())
+    _lib.check(rc, 'ddb200_crop_flags')
+    PROFILE.all_launches += 1
+    return keep, masked
+
+
+def crop_select_edges(tgt32, src32, keep, gid32=None, offset=0):
+    """The edges of a static list whose two ends are kept, original order (ddb200_crop_select_edges): ``(tgt + offset,
+    src + offset, perm, gid | None, n_dev)`` in buffers as long as the input; only the first ``n_dev[0]`` rows are live.
+    No host synchronisation."""
+    _need_cuda(tgt32, src32, keep)
+    assert tgt32.dtype == torch.int32 and src32.dtype == torch.int32 and tgt32.is_contiguous() and src32.is_contiguous()
+    assert keep.dtype == torch.bool and keep.is_contiguous()
+    if gid32 is not None:
+        assert gid32.dtype == torch.int32 and gid32.is_contiguous()
+    n, dev = tgt32.shape[0], tgt32.device
+    L = _lib.lib()
+    need = C.c_size_t(0)
+    _lib.check(L.ddb200_crop_select_edges(None, None, None, n, None, 0, None, None, None, None, None, None, C.byref(need),
+                                          _stream()), 'ddb200_crop_select_edges(size)')
+    ws = torch.empty(max(int(need.value), 1), dtype=torch.uint8, device=dev)
+    out_t, out_s, perm = (torch.empty(max(n, 1), dtype=torch.int32, device=dev) for _ in range(3))
+    out_g = torch.empty(max(n, 1), dtype=torch.int32, device=dev) if gid32 is not None else None
+    n_dev = torch.empty(1, dtype=torch.int32, device=dev)
+    have = C.c_size_t(ws.numel())
+    _lib.check(L.ddb200_crop_select_edges(_ptr(tgt32), _ptr(src32), _ptr(gid32), n, _ptr(keep), int(offset), _ptr(out_t),
+                                          _ptr(out_s), _ptr(perm), _ptr(out_g), _ptr(n_dev), _ptr(ws), C.byref(have),
+                                          _stream()), 'ddb200_crop_select_edges')
+    PROFILE.all_launches += 4
+    return out_t[:n], out_s[:n], perm[:n], out_g[:n] if out_g is not None else None, n_dev
+
+
 def csr_sort_by_target(tgt32, n_rows, want_row_ptr=False):
     """Stable device-side sort of an edge list by target: (tgt_sorted int32, perm int64, row_ptr int32 | None);
     ddb200_csr_sort_by_target with a torch-allocated workspace.  No host synchronisation."""

@@ -223,15 +223,21 @@ class GraphedSteps:
     launches (about 500 kernel launches each) with the host idle."""
 
     def __init__(self, model, g, b, coef_rows, t_rows, bond_u, bond_v, mask_u8, use_torsion, device, draw_noise,
-                 philox=None, warmup=1, consume_warmup=False):
+                 philox=None, warmup=1, consume_warmup=False, crop_rows=None):
         """``consume_warmup``: when a batch of new shapes needs an eager step before the capture, that step IS step 0 of the
-        run (``steps_done`` = 1 afterwards) instead of being thrown away - ``run(n)`` then replays the remaining n - 1."""
+        run (``steps_done`` = 1 afterwards) instead of being thrown away - ``run(n)`` then replays the remaining n - 1.
+        ``crop_rows``: the squared receptor-crop cut-off of every step (``crop_cutoff2``); the model then crops the receptor
+        on the device at each step (needs ``model.sync_free_crop_capable()``)."""
         self.g, self.b, self.device = g, b, device
         lig = g['ligand']
         self.pos = lig.pos = lig.pos.float().contiguous().clone()         # static buffer, updated in place
         self.coef = torch.tensor(coef_rows, dtype=torch.float32, device=device).contiguous()        # [steps, 6]
         self.times = torch.tensor(t_rows, dtype=torch.float32, device=device).contiguous()          # [steps, 3]
         self.step = torch.zeros(1, dtype=torch.int32, device=device)
+        self.crop = None
+        if crop_rows is not None:
+            self.crop = torch.tensor(crop_rows, dtype=torch.float32, device=device).contiguous()    # [steps]
+            g._crop = (self.crop, self.step)
         n_lig, n_rec = lig.num_nodes, g['receptor'].num_nodes
         names = ('tr', 'rot', 'tor')
 
@@ -264,7 +270,7 @@ class GraphedSteps:
         if hasattr(model, '_static'):
             model._static(g)
         sig = (b, n_lig, n_rec, int(g['ligand', 'ligand'].edge_index.shape[1]), int(g['receptor', 'receptor'].edge_index.shape[1]),
-               int(bond_u.shape[0]) if bond_u is not None else 0, draw_noise, philox is not None)
+               int(bond_u.shape[0]) if bond_u is not None else 0, draw_noise, philox is not None, crop_rows is not None)
         seen = getattr(model, '_graph_warmed_shapes', None)
         if seen is None:
             seen = set()
@@ -335,11 +341,21 @@ def _collate_any(items, device):
 def _use_cuda_graph(model, model_args, noise_fn, visualization_list, N, batch_size, cuda_graph):
     if cuda_graph is False or os.environ.get('DDB200_CUDA_GRAPH', '1') == '0':
         return False
+    crop_ok = getattr(model_args, 'crop_beyond', None) is None or \
+        (hasattr(model, 'sync_free_crop_capable') and model.sync_free_crop_capable())
     ok = (hasattr(model, 'sync_free_capable') and model.sync_free_capable() and noise_fn is None
-          and visualization_list is None and getattr(model_args, 'crop_beyond', None) is None)
+          and visualization_list is None and crop_ok)
     if cuda_graph is True and not ok:
-        raise RuntimeError("cuda_graph=True needs the sync-free model path, no noise_fn / visualization / crop_beyond")
+        raise RuntimeError("cuda_graph=True needs the sync-free model path, no noise_fn / visualization, and a model that "
+                           "crops on the device when crop_beyond is set")
     return ok
+
+
+def crop_cutoff2(t_to_sigma, t_tr, t_rot, t_tor, crop_beyond):
+    """The squared receptor-crop cut-off of a step as a float32 value: (3 sigma_tr + crop_beyond)^2 in float64
+    (utils/sampling.py:108), rounded as torch rounds a Python float compared with a float32 tensor (utils/utils.py:397)."""
+    cutoff = float(t_to_sigma(t_tr, t_rot, t_tor)[0]) * 3 + crop_beyond
+    return float(np.float32(cutoff ** 2))
 
 
 def _eager_steps(g, b, model, inference_steps, tr_schedule, rot_schedule, tor_schedule, t_schedule, t_to_sigma, model_args,
@@ -439,9 +455,13 @@ def sampling(data_list, model, inference_steps, tr_schedule, rot_schedule, tor_s
             coef_rows.append(coef)
             t_rows.append([float(tr_schedule[t_idx]), float(rot_schedule[t_idx]), float(tor_schedule[t_idx])])
         if graphed and t_schedule is None and b > 0:
+            crop_beyond = getattr(model_args, 'crop_beyond', None)
+            crop_rows = None if crop_beyond is None else [
+                crop_cutoff2(t_to_sigma, tr_schedule[i], rot_schedule[i], tor_schedule[i], crop_beyond)
+                for i in range(inference_steps)]
             steps = GraphedSteps(model, g, b, coef_rows, t_rows, bond_u, bond_v, mask_u8, use_torsion, device,
                                  draw_noise=not (ode or no_random), philox=(seed, keys) if philox else None,
-                                 consume_warmup=True)
+                                 consume_warmup=True, crop_rows=crop_rows)
             steps.run(inference_steps)
         else:
             _eager_steps(g, b, model, inference_steps, tr_schedule, rot_schedule, tor_schedule, t_schedule, t_to_sigma,

@@ -263,6 +263,31 @@ int ddb200_contact_count(const float* pos, int32_t n, float cutoff, int32_t max_
 int ddb200_contact_fill(const float* pos, int32_t n, float cutoff, int32_t max_neighbors, int32_t knn_only,
                         const int32_t* row_start, int32_t* out_nbr, int32_t* out_ctr, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Per-step receptor cropping, masked form (the receptor arrays keep their size; a dropped residue loses its edges).
+ * ddb200_crop_flags: for every residue r of complex b = rec_batch[r]
+ *   keep[r] = any over the ligand atoms j of b (segment lig_ptr[b] .. lig_ptr[b+1]) of
+ *             (lx - rx)^2 + (ly - ry)^2 + (lz - rz)^2 < cutoff2_table[*step_dev]      (step_dev NULL: row 0)
+ *   with three rounded products added left to right (no FMA) and a strict test, bit-compatible with the reference's
+ *   sum((lig - rec) ** 2, -1) < cutoff ** 2 on float32 tensors when the table holds cutoff^2 rounded to float32;
+ *   rec_pos_masked [n_rec, 3] = rec_pos, with +inf in every coordinate of a dropped residue (handed to the radius kernels
+ *   as candidates or queries, a dropped residue then has no neighbour: d^2 < r^2 is false).
+ * ddb200_crop_select_edges: the edges e of a static list (tgt / src [n_edges] receptor indices, gid [n_edges] any int32
+ *   payload, may be NULL together with out_gid) with keep[tgt[e]] && keep[src[e]], in their original order:
+ *   out_perm[k] = e, out_tgt[k] = tgt[e] + offset, out_src[k] = src[e] + offset, out_gid[k] = gid[e] for k < *n_selected;
+ *   the output arrays have n_edges rows, rows at and beyond *n_selected are unspecified; the count stays in device memory.
+ *   Workspace protocol as ddb200_csr_sort_by_target (workspace == NULL: size query).
+ * Replaces: utils/utils.py:388-413 (crop_beyond, all_atoms=False) as called at utils/sampling.py:104-109, without the
+ * deep copy / to_data_list / re-collate of the batch.
+ * ------------------------------------------------------------------------------------------------------------- */
+int ddb200_crop_flags(const float* lig_pos, const int32_t* lig_ptr, const float* rec_pos, const int32_t* rec_batch,
+                      int64_t n_rec, const float* cutoff2_table, const int32_t* step_dev, uint8_t* keep,
+                      float* rec_pos_masked, void* stream);
+int ddb200_crop_select_edges(const int32_t* tgt, const int32_t* src, const int32_t* gid, int64_t n_edges,
+                             const uint8_t* keep, int32_t offset, int32_t* out_tgt, int32_t* out_src, int32_t* out_perm,
+                             int32_t* out_gid, int32_t* n_selected, void* workspace, size_t* workspace_bytes,
+                             void* stream);
+
 #ifdef __cplusplus
 }
 #endif
