@@ -171,16 +171,13 @@ __device__ __forceinline__ void prefetch_x(const float* __restrict__ src, int cn
   }
 }
 
-// z is formed from the node values prefetched during the previous tile, then the NEXT tile's values are requested, all
-// before waiting for the accumulator tile: the gather latency overlaps the MMAs
+// z is formed from the node values prefetched during the previous tile before waiting for the accumulator tile
 template <int MULOUT, int DOUT, int ROWS>
-__device__ __forceinline__ void tile_body(const float* crow, int nch, int half, float* xn, int d_in, const float* M,
-                                          float* acc, const float* xnext, int cnt_next, int vec2, uint64_t* cfull,
-                                          uint32_t parity) {
+__device__ __forceinline__ void tile_body(const float* crow, int nch, int half, const float* xn, int d_in, const float* M,
+                                          float* acc, uint64_t* cfull, uint32_t parity) {
   float z[ROWS * DOUT];
   if (d_in == 1) make_z<1, DOUT, ROWS>(xn, M, z);
   else make_z<3, DOUT, ROWS>(xn, M, z);
-  prefetch_x(xnext, cnt_next, vec2, xn);
   mbar_wait(cfull, parity);
   consume_tile<MULOUT, DOUT, ROWS>(crow, nch, half, z, acc);
 }
@@ -189,9 +186,11 @@ __device__ __forceinline__ void tile_body(const float* crow, int nch, int half, 
 // step c < S (hi): x A hi (column block c) and x A lo (block S + c);  S <= c < 2S (lo): x A hi (block c - S);
 // c == 2S (bias): x A ones (block 2S).  Per k-block OPS_PER_KB slots of two words, stored as [A words 0-7 | B words 0-7]:
 // A word = low descriptor word of the A column block (absolute), B word = offset of the B step inside the stage in 16-byte
-// units, 0xFFFFFFFF = empty slot.
+// units; the first n slots are used.  After the MAX_KB k-blocks: n of every k-block (1 <= n <= 8 for every k-block of an
+// image: the last one holds at least the bias step).
+constexpr int SCHED_WORDS = MAX_KB * (2 * OPS_PER_KB + 1);
 __device__ __forceinline__ uint32_t a_block_offset(int c) { return (uint32_t)((c >> 2) * (A_KB_BYTES >> 4) + (c & 3) * 2); }
-__device__ __forceinline__ void build_ops(uint32_t* ops, int S, uint32_t a_lo0) {     // ops[MAX_KB][2][OPS_PER_KB]
+__device__ __forceinline__ void build_ops(uint32_t* ops, int S, uint32_t a_lo0) {     // ops[SCHED_WORDS]
   for (int kb = 0; kb < MAX_KB; ++kb) {
     uint32_t* oa = ops + kb * 2 * OPS_PER_KB;
     uint32_t* ob = oa + OPS_PER_KB;
@@ -204,7 +203,8 @@ __device__ __forceinline__ void build_ops(uint32_t* ops, int S, uint32_t a_lo0) 
       } else if (c < 2 * S) { oa[n] = a_lo0 + a_block_offset(c - S); ob[n++] = (uint32_t)j * 2; }
       else if (c == 2 * S) { oa[n] = a_lo0 + a_block_offset(2 * S); ob[n++] = (uint32_t)j * 2; }
     }
-    for (; n < OPS_PER_KB; ++n) { oa[n] = a_lo0; ob[n] = 0xFFFFFFFFu; }
+    ops[MAX_KB * 2 * OPS_PER_KB + kb] = (uint32_t)n;
+    for (; n < OPS_PER_KB; ++n) { oa[n] = a_lo0; ob[n] = 0u; }
   }
 }
 
@@ -229,69 +229,198 @@ struct Stream {
   }
 };
 
-// ---- MMA warpgroup: all k-blocks of one N tile (N = MMA width), then its epilogue: the hidden layer is
-// written back over the operand image as A' (ReLU, bf16 split), a weight tile is stored to the accumulator tile C.
-// One MMA group stays in flight while the previous k-block's stage is refilled.
-template <int N>
-__device__ __forceinline__ void mma_tile(const FusedParams& p, const Stream& st, const uint32_t* ops, int nkb, uint32_t& mc,
-                                         bool hidden, unsigned char* sA, float* sC, uint64_t* cfull, uint64_t* cempty,
-                                         uint32_t& cc, int t) {
-  float d[N / 2];
-  const uint32_t b_lo0 = gmma_desc_lo(smem_u32(st.sB));
-  for (int kb = 0; kb < nkb; ++kb, ++mc) {
-    const uint32_t s = mc % STAGES;
-    mbar_wait(&st.full[s], (mc / STAGES) & 1);
-    const uint32_t* oa = ops + kb * 2 * OPS_PER_KB;
-    const uint32_t* ob = oa + OPS_PER_KB;
-    const uint32_t b_lo = b_lo0 + s * (STAGE_BYTES >> 4);
-    uint32_t av[OPS_PER_KB], bv[OPS_PER_KB];
+// ---- MMA warpgroup.  Every product is issued MAX_N wide into one of two register sets of accumulators (Acc); k-block after
+// k-block of the CTA's B stream, counted by mc.  One MMA group stays in flight while the previous k-block's stage is
+// refilled.
+using Acc = float[MAX_N / 2];
+
+// the n MMAs of one staged k-block as one chain: one register fence in front, one commit group.  The descriptors are read
+// before the fence, so that nothing but the MMAs lies between the fence and the commit; acc0 == 0 overwrites d.
+template <int NOPS>
+__device__ __forceinline__ void mma_chain(Acc& d, const uint32_t* oa, const uint32_t* ob, uint32_t b_lo, uint32_t acc0) {
+  uint32_t a[NOPS], b[NOPS];
 #pragma unroll
-    for (int i = 0; i < OPS_PER_KB; ++i) { av[i] = oa[i]; bv[i] = ob[i] == 0xFFFFFFFFu ? ob[i] : b_lo + ob[i]; }
-    wgmma_fence();
-    Wgmma<N>::mma8(d, av, bv, (uint32_t)kb);
-    wgmma_commit();
-    if (kb > 0) {
+  for (int i = 0; i < NOPS; ++i) { a[i] = oa[i]; b[i] = b_lo + ob[i]; }
+  wgmma_fence();
+#pragma unroll
+  for (int i = 0; i < NOPS; ++i) Wgmma<MAX_N>::mma(d, gmma_desc(a[i]), gmma_desc(b[i]), i == 0 ? acc0 : 1u);
+  wgmma_commit();
+}
+
+// k-block kb of the schedule `ops` from stage mc % STAGES into d
+__device__ __forceinline__ void mma_kblock(Acc& d, const Stream& st, const uint32_t* ops, int kb, uint32_t mc) {
+  const uint32_t s = mc % STAGES;
+  mbar_wait(&st.full[s], (mc / STAGES) & 1);
+  const uint32_t* oa = ops + kb * 2 * OPS_PER_KB;
+  const uint32_t* ob = oa + OPS_PER_KB;
+  const uint32_t b_lo = gmma_desc_lo(smem_u32(st.sB)) + s * (STAGE_BYTES >> 4);
+  const uint32_t acc0 = kb != 0;
+  switch (ops[MAX_KB * 2 * OPS_PER_KB + kb]) {      // uniform: the chain length follows from the plan's shapes
+    case 1: mma_chain<1>(d, oa, ob, b_lo, acc0); break;
+    case 2: mma_chain<2>(d, oa, ob, b_lo, acc0); break;
+    case 3: mma_chain<3>(d, oa, ob, b_lo, acc0); break;
+    case 4: mma_chain<4>(d, oa, ob, b_lo, acc0); break;
+    case 5: mma_chain<5>(d, oa, ob, b_lo, acc0); break;
+    case 6: mma_chain<6>(d, oa, ob, b_lo, acc0); break;
+    case 7: mma_chain<7>(d, oa, ob, b_lo, acc0); break;
+    case 8: mma_chain<8>(d, oa, ob, b_lo, acc0); break;
+    default: __trap();     // unreachable: build_ops gives every k-block of an image 1..8 MMAs (n_kb = ceil((2S + 1) / 4))
+  }
+}
+
+// k-blocks kb0 .. nkb - 1 of one product into d.  Once a k-block is committed, every older group is waited for and the
+// previous k-block's stage refilled (for kb0 only when `release_first`: that k-block belongs to another product).
+__device__ __forceinline__ void mma_kblocks(Acc& d, const FusedParams& p, const Stream& st, const uint32_t* ops, int kb0,
+                                            int nkb, bool release_first, uint32_t& mc, int t) {
+  for (int kb = kb0; kb < nkb; ++kb, ++mc) {
+    mma_kblock(d, st, ops, kb, mc);
+    if (kb > kb0 || release_first) {
       wgmma_wait_one();
       named_bar(BAR_MMA, 128);                   // every warp is done with the previous k-block's stage
       if (t == 0) st.issue(p, mc - 1 + STAGES);
     }
   }
+}
+
+// every group complete: the last k-block's stage is refilled
+__device__ __forceinline__ void mma_drain(const FusedParams& p, const Stream& st, uint32_t mc, int t) {
   wgmma_wait_all();
-  wgmma_fence_regs(d);
   named_bar(BAR_MMA, 128);
   if (t == 0) st.issue(p, mc - 1 + STAGES);
+}
+
+// hidden layer -> A': ReLU, bf16 split, written back over the operand image; complete and visible to the async proxy
+// before the first weight-tile MMA reads it
+__device__ __forceinline__ void store_hidden(const Acc& d, const FusedParams& p, unsigned char* sA, int t) {
   const int lane = t & 31, r0 = (t >> 5) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
-  if (hidden) {
-    const int K = p.H, Kp = p.Hp;
+  const int K = p.H, Kp = p.Hp;
 #pragma unroll
-    for (int j = 0; j < N / 8; ++j)
+  for (int j = 0; j < MAX_N / 8; ++j)
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int c = 8 * j + c0, r = r0 + 8 * h;
-        __nv_bfloat16 h0, l0, h1, l1;
-        split1(fmaxf(d[4 * j + 2 * h], 0.f), h0, l0);
-        split1(fmaxf(d[4 * j + 2 * h + 1], 0.f), h1, l1);
-        if (c + 1 < K) {
-          put_a2(sA, r, c, (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16));
-          put_a2(sA, r, Kp + c, (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16));
-        } else if (c < K) {
-          put_a(sA, r, c, h0);
-          put_a(sA, r, Kp + c, l0);
+    for (int h = 0; h < 2; ++h) {
+      const int c = 8 * j + c0, r = r0 + 8 * h;
+      __nv_bfloat16 h0, l0, h1, l1;
+      split1(fmaxf(d[4 * j + 2 * h], 0.f), h0, l0);
+      split1(fmaxf(d[4 * j + 2 * h + 1], 0.f), h1, l1);
+      if (c + 1 < K) {
+        put_a2(sA, r, c, (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16));
+        put_a2(sA, r, Kp + c, (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16));
+      } else if (c < K) {
+        put_a(sA, r, c, h0);
+        put_a(sA, r, Kp + c, l0);
+      }
+    }
+  if (t < BM) put_a_tail(sA, t, K, Kp);
+  fence_proxy_async();
+  named_bar(BAR_MMA, 128);
+}
+
+// a complete weight tile -> the accumulator tile C, once the consumers have drained the previous one
+__device__ __forceinline__ void store_weights(Acc& d, float* sC, uint64_t* cfull, uint64_t* cempty, uint32_t& cc, int t) {
+  wgmma_fence_regs(d);                           // d is read only after the wait that completed it
+  const int lane = t & 31, r0 = (t >> 5) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+  mbar_wait(cempty, (cc & 1) ^ 1);
+#pragma unroll
+  for (int j = 0; j < MAX_N / 8; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      *reinterpret_cast<float2*>(sC + (r0 + 8 * h) * CLD + 8 * j + c0) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+  mbar_arrive(cfull);
+  ++cc;
+}
+
+// weight tile t, every k-block committed into `cur`, is followed by another one: that tile's first k-block is committed
+// into `nxt` first and only `cur`'s groups are waited for, so the tensor pipe works through that k-block while C is
+// written; then its remaining k-blocks are issued.
+__device__ __forceinline__ void weight_tile_next(Acc& cur, Acc& nxt, const FusedParams& p, const Stream& st,
+                                                 const uint32_t* ops, uint32_t& mc, float* sC, uint64_t* cfull,
+                                                 uint64_t* cempty, uint32_t& cc, int t) {
+  mma_kblocks(nxt, p, st, ops, 0, 1, true, mc, t);
+  store_weights(cur, sC, cfull, cempty, cc, t);
+  mma_kblocks(nxt, p, st, ops, 1, p.n_kb, true, mc, t);
+}
+
+// ---- A0' image of edge tile mt, built by all threads: [hi | lo | 1 1 0..] of [edge_attr (+ per-graph term) | node[tgt,:ns] |
+// node[src,:ns]]
+__device__ __forceinline__ void build_a0(const FusedParams& p, unsigned char* sA, long long mt, long long n_edges, int tid) {
+  const long long e0 = mt * BM;
+  const int Kin = p.K1, Kp = p.K1p;
+  if (tid < BM) put_a_tail(sA, tid, Kin, Kp);
+  if (p.a0_vec) {
+    // vector path: four threads per edge row, each converting a contiguous quarter of the row's 8-column groups (<= 5
+    // groups = 10 independent 16-byte loads).  The row's indices (attribute row, per-graph term, both end points) are
+    // loaded once per thread, then ALL data loads of the thread are issued - including the per-graph term's - then the
+    // conversions: two dependent global-memory round trips per tile.
+    constexpr int TPR = THREADS / BM;
+    const int groups = Kin >> 3, gh = (groups + TPR - 1) / TPR;
+    constexpr int PER = (144 / 8 + TPR - 1) / TPR;      // Kp <= 144 (MAX_KB k-blocks)
+    const int r = tid / TPR, g0 = (tid % TPR) * gh, g1 = min(groups, g0 + gh);
+    const long long e = e0 + r;
+    const bool live = e < n_edges;
+    const int ge = p.ne >> 3, gs = p.ns >> 3;           // groups of the attribute / of one node section
+    long long er = e;
+    int ai = -1, it = 0, is = 0;
+    if (live) {
+      if (g0 < ge) {
+        if (p.perm) er = (long long)__ldg(p.perm + e);
+        if (p.ea_add) ai = __ldg(p.ea_add_idx + e);
+      }
+      if (g0 < ge + gs && g1 > ge) it = __ldg(p.tgt + e);
+      if (g1 > ge + gs) is = __ldg(p.src + e);
+    }
+    const float* ea_row = p.ea + er * p.ld_ea;
+    const float* add_row = ai >= 0 ? p.ea_add + (long long)ai * p.ne : nullptr;
+    const float* t_row = p.node + (long long)it * p.ld_node - p.ne;
+    const float* s_row = p.node + (long long)is * p.ld_node - p.ne - p.ns;
+    float4 f[PER][2], ad[PER][2];
+#pragma unroll
+    for (int u = 0; u < PER; ++u) {
+      const int g = g0 + u, k = g << 3;
+      f[u][0] = f[u][1] = ad[u][0] = ad[u][1] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (live && g < g1) {
+        const float* src = (g < ge) ? ea_row + k : (g < ge + gs ? t_row + k : s_row + k);
+        const float4* s4 = reinterpret_cast<const float4*>(src);
+        f[u][0] = __ldg(s4);
+        f[u][1] = __ldg(s4 + 1);
+        if (g < ge && add_row) {
+          const float4* a4 = reinterpret_cast<const float4*>(add_row + k);
+          ad[u][0] = __ldg(a4);
+          ad[u][1] = __ldg(a4 + 1);
         }
       }
-    if (t < BM) put_a_tail(sA, t, K, Kp);
-    fence_proxy_async();
-    named_bar(BAR_MMA, 128);                     // A' complete before the first weight-tile MMA reads it
+    }
+#pragma unroll
+    for (int u = 0; u < PER; ++u) {
+      const int g = g0 + u;
+      if (g < g1) {
+        f[u][0].x += ad[u][0].x; f[u][0].y += ad[u][0].y; f[u][0].z += ad[u][0].z; f[u][0].w += ad[u][0].w;
+        f[u][1].x += ad[u][1].x; f[u][1].y += ad[u][1].y; f[u][1].z += ad[u][1].z; f[u][1].w += ad[u][1].w;
+        uint4 hi, lo;
+        split8(reinterpret_cast<const float*>(&f[u][0]), hi, lo);
+        put_a8(sA, r, g << 3, hi);
+        put_a8(sA, r, Kp + (g << 3), lo);
+      }
+    }
   } else {
-    mbar_wait(cempty, (cc & 1) ^ 1);             // the consumers have drained the previous tile
-#pragma unroll
-    for (int j = 0; j < N / 8; ++j)
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-        *reinterpret_cast<float2*>(sC + (r0 + 8 * h) * CLD + 8 * j + c0) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
-    mbar_arrive(cfull);
-    ++cc;
+    for (int idx = tid; idx < BM * Kin; idx += THREADS) {
+      const int r = idx / Kin, k = idx - r * Kin;
+      const long long e = e0 + r;
+      float v = 0.f;
+      if (e < n_edges) {
+        if (k < p.ne) {
+          const long long er = p.perm ? (long long)__ldg(p.perm + e) : e;
+          v = __ldg(p.ea + er * p.ld_ea + k);
+          if (p.ea_add) v += __ldg(p.ea_add + (long long)__ldg(p.ea_add_idx + e) * p.ne + k);
+        } else if (k < p.ne + p.ns) v = __ldg(p.node + (long long)__ldg(p.tgt + e) * p.ld_node + (k - p.ne));
+        else v = __ldg(p.node + (long long)__ldg(p.src + e) * p.ld_node + (k - p.ne - p.ns));
+      }
+      const __nv_bfloat16 hi = __float2bfloat16(v);
+      const __nv_bfloat16 lo = __float2bfloat16(v - __bfloat162float(hi));
+      put_a(sA, r, k, hi);
+      put_a(sA, r, Kp + k, lo);
+    }
   }
+  fence_proxy_async();
 }
 
 __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParams p) {
@@ -304,8 +433,8 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
   float* sFlush = sY + 2 * 9 * BM;                               // [4 warps][48][33] scatter staging
   float* sMtab = sFlush + 4 * 48 * FLUSH_LD;                     // [MAX_PATHS][48]
   int* sTiles = reinterpret_cast<int*>(sMtab + MAX_PATHS * MTAB);   // [MAX_TILES][8]
-  uint32_t* sOps = reinterpret_cast<uint32_t*>(sTiles + MAX_TILES * 8);   // [2][MAX_KB][2][OPS_PER_KB] MMA schedules
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sOps + 2 * MAX_KB * 2 * OPS_PER_KB);
+  uint32_t* sOps = reinterpret_cast<uint32_t*>(sTiles + MAX_TILES * 8);   // [2][SCHED_WORDS] MMA schedules
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sOps + 2 * SCHED_WORDS);
   uint64_t* full = bars;                 // B stage s has landed (TMA complete_tx)
   uint64_t* cfull = bars + STAGES;       // C holds a weight tile (128 MMA threads arrive)
   uint64_t* cempty = cfull + 1;          // the consumers have drained C (128 consumer threads arrive)
@@ -315,7 +444,7 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
   for (int i = tid; i < p.n_tiles * 8; i += THREADS) sTiles[i] = p.tiles[i];
   for (int i = tid; i < p.n_paths * MTAB; i += THREADS) sMtab[i] = p.mtab[i];
   if (tid == 32) build_ops(sOps, S1, gmma_desc_lo(smem_u32(sA)));
-  if (tid == 64) build_ops(sOps + MAX_KB * 2 * OPS_PER_KB, S2, gmma_desc_lo(smem_u32(sA)));
+  if (tid == 64) build_ops(sOps + SCHED_WORDS, S2, gmma_desc_lo(smem_u32(sA)));
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) mbar_init(&full[s], 1);
     mbar_init(cfull, 128);
@@ -330,117 +459,64 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
   if (p.n_edges_dev) { const long long nd = __ldg(p.n_edges_dev); n_edges = nd < n_edges ? (nd < 0 ? 0 : nd) : n_edges; }
   const long long n_mtiles = (n_edges + BM - 1) / BM;
   const long long my_units = blockIdx.x < n_mtiles ? (n_mtiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-  Stream st;
-  st.sB = sB; st.full = full; st.tiles = sTiles; st.n1 = n1;
-  st.per_unit = p.n_kb1 + p.n_tiles * p.n_kb;
-  st.len = (uint32_t)(my_units * st.per_unit);
-  // the ring runs ahead across edge tiles: the next tile's W1' blocks are requested while this one is contracted
-  if (tid == 0)
-    for (int i = 0; i < STAGES; ++i) st.issue(p, (uint32_t)i);
-  uint32_t mc = 0, cc = 0, cc_con = 0;
-  long long dbg_c0 = 0;
-  unsigned long long dbg_g0 = 0;
+  // debug clocks: a span is counted by subtracting its start from the counter and adding its end (modulo 2^64), so no start
+  // value is held in registers through the kernel
   if (p.dbg && blockIdx.x == 0 && tid == 0) {      // effective SM clock of this launch: clock64 ticks per globaltimer ns
-    dbg_c0 = clock64();
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(dbg_g0));
+    unsigned long long g0;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g0));
+    atomicAdd(p.dbg + 25, 0ull - (unsigned long long)clock64());
+    atomicAdd(p.dbg + 26, 0ull - g0);
   }
 
-  for (long long mt = blockIdx.x; mt < n_mtiles; mt += gridDim.x) {
-    __syncthreads();
-    const long long t_unit = p.dbg ? clock64() : 0ll;
-    // ---- A0' image: [hi | lo | 1 1 0..] of [edge_attr (+ per-graph term) | node[tgt,:ns] | node[src,:ns]] -------------
-    {
-      const long long e0 = mt * BM;
-      const int Kin = p.K1, Kp = p.K1p;
-      if (tid < BM) put_a_tail(sA, tid, Kin, Kp);
-      if (p.a0_vec) {
-        // vector path: four threads per edge row, each converting a contiguous quarter of the row's 8-column groups (<= 5
-        // groups = 10 independent 16-byte loads).  The row's indices (attribute row, per-graph term, both end points) are
-        // loaded once per thread, then ALL data loads of the thread are issued - including the per-graph term's - then the
-        // conversions: two dependent global-memory round trips per tile.
-        constexpr int TPR = THREADS / BM;
-        const int groups = Kin >> 3, gh = (groups + TPR - 1) / TPR;
-        constexpr int PER = (144 / 8 + TPR - 1) / TPR;      // Kp <= 144 (MAX_KB k-blocks)
-        const int r = tid / TPR, g0 = (tid % TPR) * gh, g1 = min(groups, g0 + gh);
-        const long long e = e0 + r;
-        const bool live = e < n_edges;
-        const int ge = p.ne >> 3, gs = p.ns >> 3;           // groups of the attribute / of one node section
-        long long er = e;
-        int ai = -1, it = 0, is = 0;
-        if (live) {
-          if (g0 < ge) {
-            if (p.perm) er = (long long)__ldg(p.perm + e);
-            if (p.ea_add) ai = __ldg(p.ea_add_idx + e);
-          }
-          if (g0 < ge + gs && g1 > ge) it = __ldg(p.tgt + e);
-          if (g1 > ge + gs) is = __ldg(p.src + e);
-        }
-        const float* ea_row = p.ea + er * p.ld_ea;
-        const float* add_row = ai >= 0 ? p.ea_add + (long long)ai * p.ne : nullptr;
-        const float* t_row = p.node + (long long)it * p.ld_node - p.ne;
-        const float* s_row = p.node + (long long)is * p.ld_node - p.ne - p.ns;
-        float4 f[PER][2], ad[PER][2];
-#pragma unroll
-        for (int u = 0; u < PER; ++u) {
-          const int g = g0 + u, k = g << 3;
-          f[u][0] = f[u][1] = ad[u][0] = ad[u][1] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (live && g < g1) {
-            const float* src = (g < ge) ? ea_row + k : (g < ge + gs ? t_row + k : s_row + k);
-            const float4* s4 = reinterpret_cast<const float4*>(src);
-            f[u][0] = __ldg(s4);
-            f[u][1] = __ldg(s4 + 1);
-            if (g < ge && add_row) {
-              const float4* a4 = reinterpret_cast<const float4*>(add_row + k);
-              ad[u][0] = __ldg(a4);
-              ad[u][1] = __ldg(a4 + 1);
-            }
-          }
-        }
-#pragma unroll
-        for (int u = 0; u < PER; ++u) {
-          const int g = g0 + u;
-          if (g < g1) {
-            f[u][0].x += ad[u][0].x; f[u][0].y += ad[u][0].y; f[u][0].z += ad[u][0].z; f[u][0].w += ad[u][0].w;
-            f[u][1].x += ad[u][1].x; f[u][1].y += ad[u][1].y; f[u][1].z += ad[u][1].z; f[u][1].w += ad[u][1].w;
-            uint4 hi, lo;
-            split8(reinterpret_cast<const float*>(&f[u][0]), hi, lo);
-            put_a8(sA, r, g << 3, hi);
-            put_a8(sA, r, Kp + (g << 3), lo);
-          }
-        }
-      } else {
-        for (int idx = tid; idx < BM * Kin; idx += THREADS) {
-          const int r = idx / Kin, k = idx - r * Kin;
-          const long long e = e0 + r;
-          float v = 0.f;
-          if (e < n_edges) {
-            if (k < p.ne) {
-              const long long er = p.perm ? (long long)__ldg(p.perm + e) : e;
-              v = __ldg(p.ea + er * p.ld_ea + k);
-              if (p.ea_add) v += __ldg(p.ea_add + (long long)__ldg(p.ea_add_idx + e) * p.ne + k);
-            } else if (k < p.ne + p.ns) v = __ldg(p.node + (long long)__ldg(p.tgt + e) * p.ld_node + (k - p.ne));
-            else v = __ldg(p.node + (long long)__ldg(p.src + e) * p.ld_node + (k - p.ne - p.ns));
-          }
-          const __nv_bfloat16 hi = __float2bfloat16(v);
-          const __nv_bfloat16 lo = __float2bfloat16(v - __bfloat162float(hi));
-          put_a(sA, r, k, hi);
-          put_a(sA, r, Kp + k, lo);
-        }
-      }
-      fence_proxy_async();
-    }
-    __syncthreads();
-
-    if (__shfl_sync(0xffffffffu, tid >> 7, 0) == 0) {     // warp-uniform for the compiler
+  // Each warpgroup runs its own loop over the CTA's edge tiles, so that the state one of them carries from tile to tile is
+  // not held in registers through the other's work (together they would not fit in 255 registers).  Both loops meet at
+  // the same two block-wide barriers per edge tile, around the A0' image that all threads build.
+  if (__shfl_sync(0xffffffffu, tid >> 7, 0) == 0) {     // warp-uniform for the compiler
+    Stream st;
+    st.sB = sB; st.full = full; st.tiles = sTiles; st.n1 = n1;
+    st.per_unit = p.n_kb1 + p.n_tiles * p.n_kb;
+    st.len = (uint32_t)(my_units * st.per_unit);
+    // the ring runs ahead across edge tiles: the next tile's W1' blocks are requested while this one is contracted
+    if (tid == 0)
+      for (int i = 0; i < STAGES; ++i) st.issue(p, (uint32_t)i);
+    uint32_t mc = 0, cc = 0;
+    for (long long mt = blockIdx.x; mt < n_mtiles; mt += gridDim.x) {
+      __syncthreads();
+      if (p.dbg && tid == 0) atomicAdd(p.dbg + 11, 0ull - (unsigned long long)clock64());
+      build_a0(p, sA, mt, n_edges, tid);
+      __syncthreads();
       // ===== MMA warpgroup: hidden layer, then every N tile.  Every product is issued MAX_N wide: the stage rows past a
-      // tile's width hold stale data whose columns are never read, and one instantiation keeps the accumulators in
-      // registers (one per width spills).
-      for (int t = -1; t < p.n_tiles; ++t) {
-        const bool hidden = t < 0;
-        mma_tile<MAX_N>(p, st, sOps + (hidden ? 0 : MAX_KB * 2 * OPS_PER_KB), hidden ? p.n_kb1 : p.n_kb, mc, hidden, sA, sC,
-                        cfull, cempty, cc, tid);
+      // tile's width hold stale data whose columns are never read, and one width keeps both accumulator sets in
+      // registers.  The tile loop is unrolled by two so that the set each tile uses is known at compile time.
+      Acc d0, d1;
+      const uint32_t* ops2 = sOps + SCHED_WORDS;
+      mma_kblocks(d0, p, st, sOps, 0, p.n_kb1, false, mc, tid);
+      mma_drain(p, st, mc, tid);
+      wgmma_fence_regs(d0);
+      store_hidden(d0, p, sA, tid);
+      mma_kblocks(d0, p, st, ops2, 0, p.n_kb, false, mc, tid);
+      for (int tile = 0;; tile += 2) {     // the last tile drains the pipe on the path that leaves the loop
+        if (tile + 1 >= p.n_tiles) {
+          mma_drain(p, st, mc, tid);
+          store_weights(d0, sC, cfull, cempty, cc, tid);
+          break;
+        }
+        weight_tile_next(d0, d1, p, st, ops2, mc, sC, cfull, cempty, cc, tid);
+        if (tile + 2 >= p.n_tiles) {
+          mma_drain(p, st, mc, tid);
+          store_weights(d1, sC, cfull, cempty, cc, tid);
+          break;
+        }
+        weight_tile_next(d1, d0, p, st, ops2, mc, sC, cfull, cempty, cc, tid);
       }
-    } else {
+      if (p.dbg && tid == 0) { atomicAdd(p.dbg + 11, (unsigned long long)clock64()); atomicAdd(p.dbg + 12, 1ull); }
+    }
+  } else {
+    uint32_t cc_con = 0;
+    for (long long mt = blockIdx.x; mt < n_mtiles; mt += gridDim.x) {
+      __syncthreads();
+      build_a0(p, sA, mt, n_edges, tid);
+      __syncthreads();
       // ===== consumers: two threads per edge (warps q and q ^ 2), each contracting alternate 32-column chunks ========
       const int q = warp & 3, half = q >> 1, ct = (q & 1) * 32 + lane;     // ct = row of the edge tile
       const long long e = mt * BM + ct;
@@ -501,12 +577,15 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
         const uint32_t par = cc_con & 1;
         const int nch = ti[1] >> 5;
         switch (kind) {
-          case 0: tile_body<48, 1, 4>(crow, nch, half, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, cfull, par); break;
-          case 1: tile_body<10, 3, 16>(crow, nch, half, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, cfull, par); break;
-          case 2: tile_body<16, 1, 8>(crow, nch, half, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, cfull, par); break;
-          default: tile_body<4, 3, 16>(crow, nch, half, xn, d_in, M, acc, xnext, cnt_next, p.x_vec2, cfull, par); break;
+          case 0: tile_body<48, 1, 4>(crow, nch, half, xn, d_in, M, acc, cfull, par); break;
+          case 1: tile_body<10, 3, 16>(crow, nch, half, xn, d_in, M, acc, cfull, par); break;
+          case 2: tile_body<16, 1, 8>(crow, nch, half, xn, d_in, M, acc, cfull, par); break;
+          default: tile_body<4, 3, 16>(crow, nch, half, xn, d_in, M, acc, cfull, par); break;
         }
         mbar_arrive(cempty);
+        // the next tile's node values are requested only now, so that they are not held in registers through the
+        // contraction; their latency overlaps the scatter and the wait for the next accumulator tile
+        prefetch_x(xnext, cnt_next, p.x_vec2, xn);
         if (flags & 2) {
           // end of an output irrep: scatter-add.  Both warps of the pair stage their 32 x nacc partial results in shared
           // memory (padded rows: conflict-free both ways); lane i of warp `half` then walks the 32 edges adding the two
@@ -543,13 +622,12 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
         if (head && valid) atomicAdd(p.cnt + dst_e, (float)run_len);
       }
     }
-    if (p.dbg && tid == 0) { atomicAdd(p.dbg + 11, (unsigned long long)(clock64() - t_unit)); atomicAdd(p.dbg + 12, 1ull); }
   }
   if (p.dbg && blockIdx.x == 0 && tid == 0) {
     unsigned long long g1;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g1));
-    atomicAdd(p.dbg + 25, (unsigned long long)(clock64() - dbg_c0));
-    atomicAdd(p.dbg + 26, g1 - dbg_g0);
+    atomicAdd(p.dbg + 25, (unsigned long long)clock64());
+    atomicAdd(p.dbg + 26, g1);
   }
 }
 
@@ -627,7 +705,7 @@ extern "C" int ddb200_fused_conv(const ddb200_fused_args* a, void* stream) {
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long n_mtiles = (a->n_edges + BM - 1) / BM;
   const size_t fixed = (BM * CLD + 2 * 9 * BM + 4 * 48 * FLUSH_LD + MAX_PATHS * MTAB) * 4 + MAX_TILES * 8 * 4 +
-                       2 * MAX_KB * 2 * OPS_PER_KB * 4 + (STAGES + 2) * sizeof(uint64_t) + 1024;
+                       2 * SCHED_WORDS * 4 + (STAGES + 2) * sizeof(uint64_t) + 1024;
   const size_t smem = (size_t)MAX_KA * A_KB_BYTES + (size_t)STAGES * STAGE_BYTES + fixed;
   if (smem > 227 * 1024) return DDB200_ESMEM;
   if (!g_dev[dev].attr_done) {      // the opt-in is a per-device attribute

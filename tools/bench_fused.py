@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of the fully fused convolution kernel alone (csrc/fused_conv.cu) on receptor-like edges of the full-width
 156 -> 156 layer: bf16 wgmma TFLOP/s issued, and - with DDB200_FUSED_DEBUG=1 - the clocks per edge tile.
-    python tools/bench_fused.py [--edges 400000] [--layer 3]"""
+    python tools/bench_fused.py [--edges 400000] [--layer 3 | --layers]"""
 import argparse
 import ctypes as C
 import json
@@ -62,23 +62,15 @@ def scan():
             del x, tgt, src, vec, ea, out, cnt
 
 
-if __name__ == '__main__':
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--scan', action='store_true', help='BASELINE config 4 size scan of the fused kernel')
-    ap.add_argument('--edges', type=int, default=400000)
-    ap.add_argument('--nodes', type=int, default=48000)
-    ap.add_argument('--deg', type=int, default=24)
-    ap.add_argument('--layer', type=int, default=3)
-    a = ap.parse_args()
-    if a.scan:
-        scan()
-        sys.exit(0)
+def layer(li, E, N, deg):
+    """Time the fused kernel on layer li's table (E edges, N nodes, `deg` edges per target); with DDB200_FUSED_DEBUG=1 also
+    the clocks per 64-edge tile against the tensor-pipe ideal and the rate at which the operand images stream from L2."""
     from diffdock_b200 import _lib, fused
     from diffdock_b200.tensor_layers import get_irrep_seq
     from diffdock_b200.tp_table import build_table
     ns = 48
     seq = get_irrep_seq(ns, 10, False, False)
-    t = build_table(seq[min(a.layer, 3)], '1x0e+1x1o+1x2e', seq[min(a.layer + 1, 3)], 'fctp')
+    t = build_table(seq[min(li, 3)], '1x0e+1x1o+1x2e', seq[min(li + 1, 3)], 'fctp')
     g = torch.Generator(device='cuda').manual_seed(0)
     H, K1 = 3 * ns, 3 * ns
     w1 = torch.randn(H, K1, device='cuda', generator=g) / K1 ** 0.5
@@ -86,9 +78,8 @@ if __name__ == '__main__':
     w2 = torch.randn(t.weight_numel, H, device='cuda', generator=g) / H ** 0.5
     b2 = torch.randn(t.weight_numel, device='cuda', generator=g) * 0.1
     plan = fused.FusedPlan(t, w1, b1, w2, b2)
-    E, N = a.edges, a.nodes
     x = torch.randn(N, t.d_in, device='cuda', generator=g)
-    tgt = (torch.arange(E, device='cuda') // a.deg).clamp_max(N - 1).int()
+    tgt = (torch.arange(E, device='cuda') // deg).clamp_max(N - 1).int()
     src = torch.randint(0, N, (E,), device='cuda', generator=g).int()
     vec = torch.randn(E, 3, device='cuda', generator=g)
     ea = torch.randn(E, ns, device='cuda', generator=g)
@@ -110,10 +101,38 @@ if __name__ == '__main__':
         ts.append(e0.elapsed_time(e1))
     ms = sorted(ts)[2]
     flops = ((E + 63) // 64) * plan.mma_flops_per_tile
-    r = {'E': E, 'tiles': plan.n_tiles, 'ms': round(ms, 3), 'bf16_issued_TFLOPs': round(flops / ms / 1e9, 1)}
+    r = {'layer': li, 'E': E, 'tiles': plan.n_tiles, 'ms': round(ms, 3), 'bf16_issued_TFLOPs': round(flops / ms / 1e9, 1)}
     if have_dbg and _lib.lib().ddb200_fused_debug_read(dbg) == 0:
         units = max(int(dbg[12]), 1)
-        r['clk_per_edge_tile'] = int(dbg[11]) // units
+        clk = int(dbg[11]) / units
+        s = 3 * ((H + 15) // 16) + 1                  # MMA steps per product (hidden layer and weight tiles alike here)
+        r['clk_per_edge_tile'] = int(clk)
+        # 4096 bf16 FLOP / clk / SM (H100 data sheet): one 64x192x16 MMA = 96 clocks
+        r['ideal_clk_per_edge_tile'] = 96 * s * (plan.n_tiles + 1)
+        r['frac_of_ideal'] = round(r['ideal_clk_per_edge_tile'] / clk, 3)
+        # operand-image bytes streamed per edge tile, as the kernel's TMA ring fetches them: the rows a product reads (W1': the
+        # padded hidden width; W2': each tile's MMA width) x 128 B per k-block
+        hp, k1p = (H + 15) // 16 * 16, (K1 + 15) // 16 * 16
+        n_kb, n_kb1 = (2 * hp + 16 + 63) // 64, (2 * k1p + 16 + 63) // 64
+        img_bytes = 128 * (n_kb1 * hp + n_kb * int(plan.tiles[:, 1].sum()))
+        r['image_B_per_clk_per_sm'] = round(img_bytes / clk, 1)
         r['edge_tiles'] = units // 5
         r['sm_clock_ghz_in_kernel'] = round(dbg[25] / max(dbg[26], 1), 3)     # clock64 ticks per globaltimer ns, CTA 0
-    print(json.dumps(r), flush=True)
+    del x, tgt, src, vec, ea, out, cnt
+    return r
+
+
+if __name__ == '__main__':
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--scan', action='store_true', help='BASELINE config 4 size scan of the fused kernel')
+    ap.add_argument('--layers', action='store_true', help='sweep the four tables of the benchmarked model (layers 0-3)')
+    ap.add_argument('--edges', type=int, default=400000)
+    ap.add_argument('--nodes', type=int, default=48000)
+    ap.add_argument('--deg', type=int, default=24)
+    ap.add_argument('--layer', type=int, default=3)
+    a = ap.parse_args()
+    if a.scan:
+        scan()
+        sys.exit(0)
+    for li in (range(4) if a.layers else [a.layer]):
+        print(json.dumps(layer(li, a.edges, a.nodes, a.deg)), flush=True)

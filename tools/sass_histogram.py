@@ -2,9 +2,8 @@
 """Static instruction histogram of the built library (cuobjdump -sass): one row per kernel with the counts of the mnemonics
 that show what the code runs on - warpgroup MMAs (HGMMA), their register fences (WARPGROUP), bulk / TMA copies (UBLKCP /
 UTMALDG), mbarrier operations (SYNCS), reductions to global memory (REDG) - and of the legacy ones it must not contain (HMMA =
-mma.sync).  Also the longest run of bf16 HGMMA separated only by uniform-datapath / move instructions, the uniform skip
-of an empty slot and the register fence before each MMA (no wgmma wait, barrier or memory access in between): the size of
-the fused kernel's MMA issue block.
+mma.sync).  Also the longest run of bf16 HGMMA separated only by uniform-datapath / move instructions (no wgmma wait,
+barrier or memory access in between): the size of the fused kernel's MMA issue block, one chain per staged k-block.
     mkdir -p build/profiles && python tools/sass_histogram.py [lib.so] > build/profiles/sass_histogram.csv"""
 import os
 import re
@@ -16,14 +15,17 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 COLS = ['HGMMA', 'WARPGROUP', 'UBLKCP', 'UTMALDG', 'SYNCS', 'ELECT', 'REDG', 'ATOMG', 'HMMA', 'FFMA', 'LDS', 'STS',
         'LDG', 'STG', 'SHFL', 'MUFU', 'UCGABAR', 'BAR']
 VARIANTS = ('HGMMA', 'WARPGROUP', 'UBLKCP', 'REDG')
-# instructions allowed between two MMAs of one issue block: predicate / uniform moves, register->uniform moves, adds, the
-# uniform skip of an empty slot and the warpgroup register fence (WARPGROUP.ARRIVE) before each MMA.  Anything else - the
-# wgmma wait (WARPGROUP.DEPBAR), a barrier, a memory access - ends the block.
+# instructions allowed between two MMAs of one issue block: the descriptor moves (uniform / register->uniform moves, adds,
+# predicate setup).  A warpgroup register fence (WARPGROUP.ARRIVE) does not end the block either, so that one injected by
+# ptxas inside a chain is seen as part of it (tests/test_fused_chain_sass_cpu.py rejects that).  Anything else - the wgmma
+# wait (WARPGROUP.DEPBAR), a barrier, a memory access - ends the block.
 GLUE = ('UMOV', 'R2UR', 'UISETP', 'IMAD', 'IADD3', 'NOP', 'UIADD3', 'LOP3', 'SHF', 'ISETP', 'P2R', 'MOV', 'PLOP3', 'BRA',
         'VOTEU', 'WARPGROUP.ARRIVE')
 
 
-def kernels(lib):
+def kernels(lib, operands=False):
+    """kernel -> its instructions' mnemonics (with `operands`: mnemonic and operands, e.g. 'HGMMA.64x192x16.F32.BF16 R24,
+    gdesc[UR4], R24, gsb0')."""
     out = subprocess.run(['cuobjdump', '-sass', lib], capture_output=True, text=True, check=True).stdout
     cur, body = None, OrderedDict()
     for line in out.splitlines():
@@ -32,9 +34,9 @@ def kernels(lib):
             cur = m.group(1)
             body[cur] = []
             continue
-        m = re.match(r'\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Za-z0-9_.]*)', line)
+        m = re.match(r'\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Za-z0-9_.]*)([^;]*)', line)
         if m and cur is not None:
-            body[cur].append(m.group(1))
+            body[cur].append(m.group(1) + m.group(2).rstrip() if operands else m.group(1))
     return body
 
 
