@@ -1,18 +1,19 @@
 // Fully fused equivariant convolution for one edge group (sm_90a): radial MLP on the Hopper tensor cores (wgmma) +
 // tensor-product contraction + scatter - the per-edge weight tensor [E, weight_numel] never exists in HBM.
 //
-//   for a tile of 64 CSR-sorted edges (one CTA, persistent over tiles; warpgroup 0 multiplies, warpgroup 1 contracts):
-//     A0' = split-bf16([edge_attr (+ per-graph term) | node[tgt,:ns] | node[src,:ns]])   built in shared memory (128B swizzle)
+//   for a tile of 128 CSR-sorted edges (one CTA, persistent over tiles; warpgroup g owns edges 64 g .. 64 g + 63 and does
+//   all of their work; the B' images are streamed once per CTA by TMA bulk copies through a 3-stage ring both read):
+//     A0' = split-bf16([edge_attr (+ per-graph term) | node[tgt,:ns] | node[src,:ns]])   the warpgroup's own image in shared
+//                                      memory (128B swizzle)
 //     H   = relu(A0' x W1'^T)          wgmma -> registers -> A' image (bias folded via two constant-one columns)
 //     for every N tile (whole rows u of one path block [mul_in, mul_out], <= 192 columns):
-//        Wt = A' x W2'^T[tile]         wgmma m64nNk16 into registers (B' images streamed by TMA bulk copies through a
-//                                      4-stage ring), then stored to a padded shared-memory tile C [64][196] once the
-//                                      consumers have drained the previous one: the next tile's MMAs overlap the contraction
-//        consumer thread pair (e, half): acc[w,k] += Wt[e, (u,w)] * z_e[u,k] over its half of the 32-column chunks,
-//                                        z_e[u,k] = sum_i x[src_e][u,i] M_e[i,k],  M_e = edge_weight * coef * C . Y(vec_e)
-//     at the end of an output irrep: sum[tgt_e, irrep] += acc  (the pair's partial sums are added and runs of equal
-//                                                              targets reduced through shared memory, then one coalesced
-//                                                              RED.ADD per run and 32 output values)
+//        z_e[u,k] = sum_i x[src_e][u,i] M_e[i,k],  M_e = edge_weight * coef * C . Y(vec_e)   built by each quad of threads
+//                                      for its two edges in a per-warpgroup shared-memory buffer
+//        Wt = A' x W2'^T[tile]         wgmma m64nNk16 into registers
+//        acc[w,k] += Wt[e, (u,w)] * z_e[u,k]   straight from the accumulator registers (partial sums per thread)
+//     at the end of an output irrep: sum[tgt_e, irrep] += acc  (the partial sums are staged in shared memory, runs of
+//                                                              equal targets reduced, then one coalesced RED.ADD per run
+//                                                              and output value)
 //
 // Operand layout: BOTH operand images hold each split part once - activation [hi | lo | 1 1 0..], static operand
 // [hi | lo | b_hi b_lo 0..] (2 Kp + 16 columns, Kp = K rounded up to 16).  The three products hi.hi + hi.lo + lo.hi (+ bias)
@@ -36,21 +37,25 @@ namespace {
 
 using namespace ddb200_sm90;
 
-constexpr int BM = 64, BK = 64;                  // CTA tile = one wgmma M; BK bf16 = one 128-byte swizzle row
+constexpr int BM = 64, BK = 64;                  // edges of one warpgroup = one wgmma M; BK bf16 = one 128-byte swizzle row
+constexpr int CTA_EDGES = 2 * BM;                // edge tile of the CTA: one 64-edge half per warpgroup
 constexpr int A_KB_BYTES = BM * BK * 2;          // 8 KB
 constexpr int B_IMAGE_BYTES = 256 * BK * 2;      // 32 KB: one k-block image of an N tile in global memory
 constexpr int MAX_N = 192;                       // widest N tile of a plan (and widest hidden layer)
-constexpr int STAGES = 4;
+constexpr int STAGES = 4;                        // every stage feeds both warpgroups' chains
 constexpr int STAGE_BYTES = MAX_N * BK * 2;      // 24 KB: the rows of an image the MMA reads
 constexpr int MAX_KB = 5;                        // k-blocks of either operand image: 2 Kp + 16 <= 320  (Kp <= 144)
 constexpr int MAX_KA = MAX_KB;
+constexpr int A_IMAGE_BYTES = MAX_KA * A_KB_BYTES;    // 40 KB: one warpgroup's activation image
 constexpr int OPS_PER_KB = 8;                    // MMAs that read one staged k-block of B (4 steps x up to 2 A partners)
-constexpr int THREADS = 256;                     // warpgroup 0: MMA, warpgroup 1: consumers (two threads per edge)
+constexpr int THREADS = 256;                     // two warpgroups, each with its own 64 edges
 constexpr int MAX_TILES = 128, MAX_PATHS = 16, MTAB = 48;     // per path: dense [3][3][5] table, padded to 48 floats
-constexpr int FLUSH_LD = 33;                     // padded row of the per-warp scatter staging buffer [48][33]
-constexpr int CLD = 196;                         // row of the accumulator tile: 16-byte reads of 8 rows hit 8 bank groups
-constexpr int BAR_MMA = 1, BAR_PAIR = 2;         // named barriers: the MMA warpgroup, the two consumer warp pairs
+constexpr int BAR_WG = 1;                        // named barrier BAR_WG + g: the 128 threads of warpgroup g
 
+// fire-and-forget global reduction (atomicAdd here may be compiled to an atomic that returns its old value)
+__device__ __forceinline__ void red_add(float* addr, float v) {
+  asm volatile("red.global.add.f32 [%0], %1;" ::"l"(addr), "f"(v) : "memory");
+}
 __device__ __forceinline__ void wgmma_wait_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 __device__ __forceinline__ void put_a(unsigned char* sA, int r, int col, __nv_bfloat16 v) {
@@ -114,49 +119,76 @@ struct FusedParams {
   unsigned long long* dbg;                           // optional [32] clock counters (DDB200_FUSED_DEBUG=1), else nullptr
 };
 
-// ---- consumer: this thread's half (alternate 32-column chunks) of one accumulator tile (ROWS rows u of a [mul_in, MULOUT]
-// block) times z -> acc.  Only the first `nch` chunks hold MMA results (the last tile of a path block may be narrower).
+// ---- contraction straight from the wgmma accumulators.  Thread t of a warpgroup holds rows r0 = 16 (t / 32) + (t % 32) / 4
+// and r0 + 8 (its two edges h = 0, 1) and columns c = 8 j + 2 q + b (q = t % 4, b = 0, 1) of the weight tile as
+// d[4 j + 2 h + b]; column c is row u = c / MULOUT and output channel w = c % MULOUT of the tile.  The thread keeps its
+// partial sums per slot (j mod P, b), P = MULOUT / gcd(MULOUT, 8): the slots of one thread hold distinct channels (slot ->
+// channel is fixed up to a shift by 2 q, so every index into the partial sums is known at compile time), and NCOPY =
+// 8 / gcd(MULOUT, 8) threads of a quad hold partial sums of the same channel.
+template <int MULOUT> struct Slots {
+  static_assert(MULOUT % 2 == 0, "a column pair (b = 0, 1) lies in one row u");
+  static constexpr int G = MULOUT % 8 == 0 ? 8 : (MULOUT % 4 == 0 ? 4 : 2);
+  static constexpr int P = MULOUT / G, N = 2 * P, NCOPY = 8 / G;
+  static __device__ __forceinline__ int w(int slot, int q) { return (8 * (slot >> 1) + 2 * q + (slot & 1)) % MULOUT; }
+};
+constexpr int NACC_MAX = 60;                     // partial sums per thread: slots x d_out x 2 edges, at most 10 x 3 x 2
+constexpr int ZLD = 68;                          // z buffer row of one edge: [16 rows u][4]; 8 edges' 16-byte reads hit 8 bank groups
+constexpr int WG_BUF = 64 * ZLD;                 // floats per warpgroup: z [64][ZLD], or the scatter staging [copies][64][nacc + 1]
+
+using Acc = float[MAX_N / 2];
+
+// acc[(slot d_out + k) 2 + h] += d[edge h, columns of the slot] * z[edge h][u][k] over the tile's first `nch` 32-column
+// chunks; z = the row of this thread's first edge in the z buffer (the second edge lies 8 rows further)
 template <int MULOUT, int DOUT, int ROWS>
-__device__ __forceinline__ void consume_tile(const float* __restrict__ crow, int nch, int half, const float* __restrict__ z,
-                                             float* __restrict__ acc) {
+__device__ __forceinline__ void contract(const Acc& d, const float* __restrict__ z, int nch, int q, float* __restrict__ acc) {
+  using S = Slots<MULOUT>;
   constexpr int NCOL = MULOUT * ROWS;
-  static_assert(NCOL % 32 == 0 && NCOL <= MAX_N, "tile width");
+  static_assert(NCOL % 32 == 0 && NCOL <= MAX_N && S::N * DOUT * 2 <= NACC_MAX, "tile width");
 #pragma unroll
-  for (int c = 0; c < NCOL / 32; ++c) {
-    if (c < nch && (c & 1) == half) {
-      float v[32];
+  for (int j = 0; j < NCOL / 8; ++j) {
+    if ((j >> 2) < nch) {
+      const int u = (MULOUT % 8 == 0) ? j / (MULOUT / 8) : (8 * j + 2 * q) / MULOUT;
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float4 f = reinterpret_cast<const float4*>(crow + c * 32)[q];
-        v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
-      }
+      for (int h = 0; h < 2; ++h) {
+        float zk[3];
+        if (DOUT == 1) {
+          zk[0] = z[h * 8 * ZLD + u * 4];
+        } else {
+          const float4 v = *reinterpret_cast<const float4*>(z + h * 8 * ZLD + u * 4);
+          zk[0] = v.x; zk[1] = v.y; zk[2] = v.z;
+        }
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int col = c * 32 + j, row = col / MULOUT, w = col % MULOUT;     // compile-time after unrolling
+        for (int b = 0; b < 2; ++b) {
+          const int slot = (j % S::P) * 2 + b;
 #pragma unroll
-        for (int k = 0; k < DOUT; ++k) acc[w * DOUT + k] = fmaf(v[j], z[row * DOUT + k], acc[w * DOUT + k]);
+          for (int k = 0; k < DOUT; ++k)
+            acc[(slot * DOUT + k) * 2 + h] = fmaf(d[4 * j + 2 * h + b], zk[k], acc[(slot * DOUT + k) * 2 + h]);
+        }
       }
     }
   }
 }
 
-// z[r, k] = sum_i x[x_off + r*DIN + i] * M[i, k] for the tile's rows; xv = the tile's gathered node values (prefetched into
-// registers one tile ahead, zero beyond the valid rows)
-template <int DIN, int DOUT, int ROWS>
-__device__ __forceinline__ void make_z(const float* __restrict__ xv, const float* __restrict__ M, float* __restrict__ z) {
+// z[u][k] = sum_i x[u d_in + i] M[i][k] for this thread's edge and the tile rows u0 .. u0 + 7 (< ROWS), into its row `zrow`
+// of the z buffer; xn = the node values of these rows, prefetched one tile ahead (zero past the tile's rows)
+template <int DOUT, int ROWS>
+__device__ __forceinline__ void build_z(const float* __restrict__ xn, int d_in, const float* __restrict__ M,
+                                        float* __restrict__ zrow, int u0) {
+  constexpr int NU = ROWS < 8 ? ROWS : 8;
+  if (u0 >= ROWS) return;
 #pragma unroll
-  for (int r = 0; r < ROWS; ++r) {
+  for (int r = 0; r < NU; ++r) {
+    float z[3] = {0.f, 0.f, 0.f};
 #pragma unroll
     for (int k = 0; k < DOUT; ++k) {
-      float a = 0.f;
-#pragma unroll
-      for (int i = 0; i < DIN; ++i) a = fmaf(xv[r * DIN + i], M[i * 3 + k], a);
-      z[r * DOUT + k] = a;
+      if (d_in == 1) z[k] = xn[r] * M[k];
+      else z[k] = fmaf(xn[3 * r + 2], M[6 + k], fmaf(xn[3 * r + 1], M[3 + k], xn[3 * r] * M[k]));
     }
+    *reinterpret_cast<float4*>(zrow + (u0 + r) * 4) = make_float4(z[0], z[1], z[2], 0.f);
   }
 }
 
-constexpr int XN = 48;     // gathered node values of one tile: at most 16 rows x 3 components
+constexpr int XN = 24;     // node values one thread gathers per tile: 8 rows x at most 3 components
 __device__ __forceinline__ void prefetch_x(const float* __restrict__ src, int cnt, int vec2, float* __restrict__ xn) {
   if (vec2) {          // 8-byte loads: every tile offset and count of the plan is even
 #pragma unroll
@@ -170,24 +202,81 @@ __device__ __forceinline__ void prefetch_x(const float* __restrict__ src, int cn
     for (int j = 0; j < XN; ++j) xn[j] = (j < cnt) ? __ldg(src + j) : 0.f;
   }
 }
+// node values of tile `ti`'s rows u0 .. u0 + 7 for the source row xrow
+__device__ __forceinline__ void prefetch_tile(const float* xrow, const int* ti, int u0, int vec2, float* xn) {
+  const int d_in = ti[4], rows = min(max(ti[3] - u0, 0), 8);
+  prefetch_x(xrow + ti[2] + u0 * d_in, rows * d_in, vec2, xn);
+}
 
-// z is formed from the node values prefetched during the previous tile before waiting for the accumulator tile
-template <int MULOUT, int DOUT, int ROWS>
-__device__ __forceinline__ void tile_body(const float* crow, int nch, int half, const float* xn, int d_in, const float* M,
-                                          float* acc, uint64_t* cfull, uint32_t parity) {
-  float z[ROWS * DOUT];
-  if (d_in == 1) make_z<1, DOUT, ROWS>(xn, M, z);
-  else make_z<3, DOUT, ROWS>(xn, M, z);
-  mbar_wait(cfull, parity);
-  consume_tile<MULOUT, DOUT, ROWS>(crow, nch, half, z, acc);
+// End of an output irrep: scatter-add of the warpgroup's 64 edges.  Every thread stages its partial sums in shared memory
+// (over the z buffer, at most two copies: with four, the pairs q, q ^ 1 are first added by a shuffle); warp w4 then takes edges 32 (w4 & 1) .. + 31 and output value i = 32 (w4 >> 1) + lane,
+// adds the copies, sums runs of equal targets (CSR order makes them contiguous; unsorted input just yields runs of length
+// one) and issues ONE fully coalesced RED.ADD per run for output value i.
+template <int MULOUT, int DOUT>
+__device__ __forceinline__ void flush(const FusedParams& p, float* __restrict__ acc, float* buf, int r0, int q, int w4,
+                                      int lane, int dst_s, uint32_t head_mask, int out_off, int bar) {
+  using S = Slots<MULOUT>;
+  constexpr int NACC = MULOUT * DOUT, LD = NACC + 1, NCOPY = S::NCOPY == 4 ? 2 : S::NCOPY;
+  static_assert(NCOPY * 64 * LD <= WG_BUF, "staging area");
+  bool writes = true;
+  if constexpr (S::NCOPY == 4) {
+    // slot (j + 1) mod 5 of thread q + 1 holds the channel of slot j of thread q (8 = -2 mod 10): the even threads add
+    // their odd partner's partial sums and stage them, the odd ones stage nothing
+    static_assert(MULOUT == 10 && S::P == 5, "quad reduction");
+    const bool odd = q & 1;
+    writes = !odd;
+#pragma unroll
+    for (int j = 0; j < 5; ++j)
+#pragma unroll
+      for (int b = 0; b < 2; ++b)
+#pragma unroll
+        for (int k = 0; k < DOUT; ++k)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int own = ((j * 2 + b) * DOUT + k) * 2 + h;
+            const int up = ((((j + 1) % 5) * 2 + b) * DOUT + k) * 2 + h;
+            const float r = __shfl_xor_sync(0xffffffffu, odd ? acc[up] : 0.f, 1);
+            if (!odd) acc[own] += r;
+          }
+  }
+  named_bar(bar, 128);                           // every warp is done with its z rows
+  float* st = buf + (NCOPY == 1 ? 0 : q >> 1) * 64 * LD;
+  if (writes) {
+#pragma unroll
+    for (int slot = 0; slot < S::N; ++slot) {
+      const int w = S::w(slot, q);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int k = 0; k < DOUT; ++k) st[(r0 + 8 * h) * LD + w * DOUT + k] = acc[(slot * DOUT + k) * 2 + h];
+    }
+  }
+  named_bar(bar, 128);
+  const int half = w4 >> 1, i = 32 * half + lane;
+  if (32 * half < NACC) {
+    const bool act = i < NACC;
+    const float* col = buf + 32 * (w4 & 1) * LD + (act ? i : 0);
+    float s = 0.f;
+#pragma unroll
+    for (int le = 0; le < 32; ++le) {
+#pragma unroll
+      for (int c = 0; c < NCOPY; ++c) s += col[(c * 64 + le) * LD];
+      if (le == 31 || ((head_mask >> (le + 1)) & 1)) {          // warp-uniform: last edge of a run
+        const int dst = __shfl_sync(0xffffffffu, dst_s, le);
+        if (dst >= 0 && act) red_add(p.sum + (long long)dst * p.d_out + out_off + i, s);
+        s = 0.f;
+      }
+    }
+  }
+  named_bar(bar, 128);                           // the staging area is free for the next z rows
 }
 
 // MMA schedule of one staged k-block of B (4 steps of 16 columns; images [hi | lo | bias], S = Kp / 16 steps per part):
 // step c < S (hi): x A hi (column block c) and x A lo (block S + c);  S <= c < 2S (lo): x A hi (block c - S);
 // c == 2S (bias): x A ones (block 2S).  Per k-block OPS_PER_KB slots of two words, stored as [A words 0-7 | B words 0-7]:
-// A word = low descriptor word of the A column block (absolute), B word = offset of the B step inside the stage in 16-byte
-// units; the first n slots are used.  After the MAX_KB k-blocks: n of every k-block (1 <= n <= 8 for every k-block of an
-// image: the last one holds at least the bias step).
+// A word = low descriptor word of the A column block (absolute: one schedule per warpgroup image), B word = offset of the B step
+// inside the stage in 16-byte units; the first n slots are used.  After the MAX_KB k-blocks: n of every k-block
+// (1 <= n <= 8 for every k-block of an image: the last one holds at least the bias step).
 constexpr int SCHED_WORDS = MAX_KB * (2 * OPS_PER_KB + 1);
 __device__ __forceinline__ uint32_t a_block_offset(int c) { return (uint32_t)((c >> 2) * (A_KB_BYTES >> 4) + (c & 3) * 2); }
 __device__ __forceinline__ void build_ops(uint32_t* ops, int S, uint32_t a_lo0) {     // ops[SCHED_WORDS]
@@ -208,9 +297,10 @@ __device__ __forceinline__ void build_ops(uint32_t* ops, int S, uint32_t a_lo0) 
   }
 }
 
-// B stream of a CTA: per edge tile the W1' k-blocks, then every N tile's W2' k-blocks; item i goes to stage i % STAGES
+// B stream of a CTA: per edge tile the W1' k-blocks, then every N tile's W2' k-blocks; item i goes to stage i % STAGES and
+// is read by both warpgroups
 struct Stream {
-  unsigned char* sB; uint64_t* full; const int* tiles;
+  unsigned char* sB; uint64_t* full; uint32_t* rel; const int* tiles;
   int n1, per_unit; uint32_t len;
   __device__ __forceinline__ void issue(const FusedParams& p, uint32_t i) const {
     if (i >= len) return;
@@ -227,71 +317,79 @@ struct Stream {
     const uint32_t s = i % STAGES;
     bulk_load(sB + (size_t)s * STAGE_BYTES, src, bytes, &full[s]);
   }
+  // item i has been read by every MMA of this warpgroup (its group is complete in every warp): the second warpgroup to
+  // release it refills its stage with item i + STAGES (rel[s] counts two releases per use of stage s)
+  __device__ __forceinline__ void release(const FusedParams& p, uint32_t i, int bar, int t) const {
+    named_bar(bar, 128);
+    if (t == 0) {
+      __threadfence_block();
+      if (atomicAdd(rel + i % STAGES, 1u) & 1u) issue(p, i + STAGES);
+    }
+  }
 };
 
-// ---- MMA warpgroup.  Every product is issued MAX_N wide into one of two register sets of accumulators (Acc); k-block after
-// k-block of the CTA's B stream, counted by mc.  One MMA group stays in flight while the previous k-block's stage is
-// refilled.
-using Acc = float[MAX_N / 2];
+// ---- MMAs of a warpgroup.  Every product is issued MAX_N wide into the warpgroup's 96 accumulators, k-block after k-block
+// of the CTA's B stream, counted by mc.
 
 // the n MMAs of one staged k-block as one chain: one register fence in front, one commit group.  The descriptors are read
-// before the fence, so that nothing but the MMAs lies between the fence and the commit; acc0 == 0 overwrites d.
-template <int NOPS>
-__device__ __forceinline__ void mma_chain(Acc& d, const uint32_t* oa, const uint32_t* ob, uint32_t b_lo, uint32_t acc0) {
+// before the fence, so that nothing but the MMAs lies between the fence and the commit.  The first MMA of a product
+// (FIRST) overwrites d and does not read it: the accumulators are dead between products.
+template <int NOPS, bool FIRST>
+__device__ __forceinline__ void mma_chain(Acc& d, const uint32_t* oa, const uint32_t* ob, uint32_t b_lo) {
   uint32_t a[NOPS], b[NOPS];
 #pragma unroll
   for (int i = 0; i < NOPS; ++i) { a[i] = oa[i]; b[i] = b_lo + ob[i]; }
   wgmma_fence();
 #pragma unroll
-  for (int i = 0; i < NOPS; ++i) Wgmma<MAX_N>::mma(d, gmma_desc(a[i]), gmma_desc(b[i]), i == 0 ? acc0 : 1u);
+  for (int i = 0; i < NOPS; ++i) {
+    if (FIRST && i == 0) wgmma192_first(d, gmma_desc(a[i]), gmma_desc(b[i]));
+    else Wgmma<MAX_N>::mma(d, gmma_desc(a[i]), gmma_desc(b[i]), 1u);
+  }
   wgmma_commit();
 }
 
-// k-block kb of the schedule `ops` from stage mc % STAGES into d
-__device__ __forceinline__ void mma_kblock(Acc& d, const Stream& st, const uint32_t* ops, int kb, uint32_t mc) {
+// k-block kb of the schedule `ops` from stage mc % STAGES into d; dwait (debug, one thread per warpgroup) collects the
+// clocks spent waiting for the stage to land
+template <bool FIRST>
+__device__ __forceinline__ void mma_kblock(Acc& d, const Stream& st, const uint32_t* ops, int kb, uint32_t mc,
+                                           unsigned long long* dwait) {
   const uint32_t s = mc % STAGES;
+  const long long c0 = dwait ? clock64() : 0;
   mbar_wait(&st.full[s], (mc / STAGES) & 1);
+  if (dwait) *dwait += (unsigned long long)(clock64() - c0);
   const uint32_t* oa = ops + kb * 2 * OPS_PER_KB;
   const uint32_t* ob = oa + OPS_PER_KB;
   const uint32_t b_lo = gmma_desc_lo(smem_u32(st.sB)) + s * (STAGE_BYTES >> 4);
-  const uint32_t acc0 = kb != 0;
   switch (ops[MAX_KB * 2 * OPS_PER_KB + kb]) {      // uniform: the chain length follows from the plan's shapes
-    case 1: mma_chain<1>(d, oa, ob, b_lo, acc0); break;
-    case 2: mma_chain<2>(d, oa, ob, b_lo, acc0); break;
-    case 3: mma_chain<3>(d, oa, ob, b_lo, acc0); break;
-    case 4: mma_chain<4>(d, oa, ob, b_lo, acc0); break;
-    case 5: mma_chain<5>(d, oa, ob, b_lo, acc0); break;
-    case 6: mma_chain<6>(d, oa, ob, b_lo, acc0); break;
-    case 7: mma_chain<7>(d, oa, ob, b_lo, acc0); break;
-    case 8: mma_chain<8>(d, oa, ob, b_lo, acc0); break;
+    case 1: mma_chain<1, FIRST>(d, oa, ob, b_lo); break;
+    case 2: mma_chain<2, FIRST>(d, oa, ob, b_lo); break;
+    case 3: mma_chain<3, FIRST>(d, oa, ob, b_lo); break;
+    case 4: mma_chain<4, FIRST>(d, oa, ob, b_lo); break;
+    case 5: mma_chain<5, FIRST>(d, oa, ob, b_lo); break;
+    case 6: mma_chain<6, FIRST>(d, oa, ob, b_lo); break;
+    case 7: mma_chain<7, FIRST>(d, oa, ob, b_lo); break;
+    case 8: mma_chain<8, FIRST>(d, oa, ob, b_lo); break;
     default: __trap();     // unreachable: build_ops gives every k-block of an image 1..8 MMAs (n_kb = ceil((2S + 1) / 4))
   }
 }
 
-// k-blocks kb0 .. nkb - 1 of one product into d.  Once a k-block is committed, every older group is waited for and the
-// previous k-block's stage refilled (for kb0 only when `release_first`: that k-block belongs to another product).
-__device__ __forceinline__ void mma_kblocks(Acc& d, const FusedParams& p, const Stream& st, const uint32_t* ops, int kb0,
-                                            int nkb, bool release_first, uint32_t& mc, int t) {
-  for (int kb = kb0; kb < nkb; ++kb, ++mc) {
-    mma_kblock(d, st, ops, kb, mc);
-    if (kb > kb0 || release_first) {
-      wgmma_wait_one();
-      named_bar(BAR_MMA, 128);                   // every warp is done with the previous k-block's stage
-      if (t == 0) st.issue(p, mc - 1 + STAGES);
-    }
+// one product, k-blocks 0 .. nkb - 1, into d.  Once a k-block is committed the previous one is waited for and released;
+// on return every group is complete, every stage the product read released and d readable.
+__device__ __forceinline__ void mma_product(Acc& d, const FusedParams& p, const Stream& st, const uint32_t* ops, int nkb, uint32_t& mc, int bar, int t, unsigned long long* dwait) {
+  mma_kblock<true>(d, st, ops, 0, mc++, dwait);
+  for (int kb = 1; kb < nkb; ++kb, ++mc) {
+    mma_kblock<false>(d, st, ops, kb, mc, dwait);
+    wgmma_wait_one();
+    st.release(p, mc - 1, bar, t);
   }
-}
-
-// every group complete: the last k-block's stage is refilled
-__device__ __forceinline__ void mma_drain(const FusedParams& p, const Stream& st, uint32_t mc, int t) {
   wgmma_wait_all();
-  named_bar(BAR_MMA, 128);
-  if (t == 0) st.issue(p, mc - 1 + STAGES);
+  st.release(p, mc - 1, bar, t);
+  wgmma_fence_regs(d);                           // d is read only after the wait that completed it
 }
 
-// hidden layer -> A': ReLU, bf16 split, written back over the operand image; complete and visible to the async proxy
-// before the first weight-tile MMA reads it
-__device__ __forceinline__ void store_hidden(const Acc& d, const FusedParams& p, unsigned char* sA, int t) {
+// hidden layer -> A': ReLU, bf16 split, written back over the warpgroup's operand image; complete and visible to the async
+// proxy before the first weight-tile MMA reads it
+__device__ __forceinline__ void store_hidden(const Acc& d, const FusedParams& p, unsigned char* sA, int t, int bar) {
   const int lane = t & 31, r0 = (t >> 5) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
   const int K = p.H, Kp = p.Hp;
 #pragma unroll
@@ -312,97 +410,74 @@ __device__ __forceinline__ void store_hidden(const Acc& d, const FusedParams& p,
     }
   if (t < BM) put_a_tail(sA, t, K, Kp);
   fence_proxy_async();
-  named_bar(BAR_MMA, 128);
+  named_bar(bar, 128);
 }
 
-// a complete weight tile -> the accumulator tile C, once the consumers have drained the previous one
-__device__ __forceinline__ void store_weights(Acc& d, float* sC, uint64_t* cfull, uint64_t* cempty, uint32_t& cc, int t) {
-  wgmma_fence_regs(d);                           // d is read only after the wait that completed it
-  const int lane = t & 31, r0 = (t >> 5) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
-  mbar_wait(cempty, (cc & 1) ^ 1);
-#pragma unroll
-  for (int j = 0; j < MAX_N / 8; ++j)
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-      *reinterpret_cast<float2*>(sC + (r0 + 8 * h) * CLD + 8 * j + c0) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
-  mbar_arrive(cfull);
-  ++cc;
-}
-
-// weight tile t, every k-block committed into `cur`, is followed by another one: that tile's first k-block is committed
-// into `nxt` first and only `cur`'s groups are waited for, so the tensor pipe works through that k-block while C is
-// written; then its remaining k-blocks are issued.
-__device__ __forceinline__ void weight_tile_next(Acc& cur, Acc& nxt, const FusedParams& p, const Stream& st,
-                                                 const uint32_t* ops, uint32_t& mc, float* sC, uint64_t* cfull,
-                                                 uint64_t* cempty, uint32_t& cc, int t) {
-  mma_kblocks(nxt, p, st, ops, 0, 1, true, mc, t);
-  store_weights(cur, sC, cfull, cempty, cc, t);
-  mma_kblocks(nxt, p, st, ops, 1, p.n_kb, true, mc, t);
-}
-
-// ---- A0' image of edge tile mt, built by all threads: [hi | lo | 1 1 0..] of [edge_attr (+ per-graph term) | node[tgt,:ns] |
-// node[src,:ns]]
-__device__ __forceinline__ void build_a0(const FusedParams& p, unsigned char* sA, long long mt, long long n_edges, int tid) {
-  const long long e0 = mt * BM;
+// ---- A0' image of the warpgroup's 64 edges e0 .. e0 + 63, built by its 128 threads: [hi | lo | 1 1 0..] of
+// [edge_attr (+ per-graph term) | node[tgt,:ns] | node[src,:ns]]
+__device__ __forceinline__ void build_a0(const FusedParams& p, unsigned char* sA, long long e0, long long n_edges, int t) {
   const int Kin = p.K1, Kp = p.K1p;
-  if (tid < BM) put_a_tail(sA, tid, Kin, Kp);
+  if (t < BM) put_a_tail(sA, t, Kin, Kp);
   if (p.a0_vec) {
-    // vector path: four threads per edge row, each converting a contiguous quarter of the row's 8-column groups (<= 5
-    // groups = 10 independent 16-byte loads).  The row's indices (attribute row, per-graph term, both end points) are
-    // loaded once per thread, then ALL data loads of the thread are issued - including the per-graph term's - then the
-    // conversions: two dependent global-memory round trips per tile.
-    constexpr int TPR = THREADS / BM;
+    // vector path: four (virtual) threads per edge row, each converting a contiguous quarter of the row's 8-column groups
+    // (<= 5 groups = 10 independent 16-byte loads); the 128 threads take two passes over the 64 rows.  The row's indices
+    // (attribute row, per-graph term, both end points) are loaded once per pass, then ALL data loads of the pass are
+    // issued - including the per-graph term's - then the conversions: two dependent global-memory round trips per pass.
+    constexpr int TPR = 4;
     const int groups = Kin >> 3, gh = (groups + TPR - 1) / TPR;
     constexpr int PER = (144 / 8 + TPR - 1) / TPR;      // Kp <= 144 (MAX_KB k-blocks)
-    const int r = tid / TPR, g0 = (tid % TPR) * gh, g1 = min(groups, g0 + gh);
-    const long long e = e0 + r;
-    const bool live = e < n_edges;
-    const int ge = p.ne >> 3, gs = p.ns >> 3;           // groups of the attribute / of one node section
-    long long er = e;
-    int ai = -1, it = 0, is = 0;
-    if (live) {
-      if (g0 < ge) {
-        if (p.perm) er = (long long)__ldg(p.perm + e);
-        if (p.ea_add) ai = __ldg(p.ea_add_idx + e);
+#pragma unroll 1
+    for (int vt = t; vt < BM * TPR; vt += 128) {
+      const int r = vt / TPR, g0 = (vt % TPR) * gh, g1 = min(groups, g0 + gh);
+      const long long e = e0 + r;
+      const bool live = e < n_edges;
+      const int ge = p.ne >> 3, gs = p.ns >> 3;           // groups of the attribute / of one node section
+      long long er = e;
+      int ai = -1, it = 0, is = 0;
+      if (live) {
+        if (g0 < ge) {
+          if (p.perm) er = (long long)__ldg(p.perm + e);
+          if (p.ea_add) ai = __ldg(p.ea_add_idx + e);
+        }
+        if (g0 < ge + gs && g1 > ge) it = __ldg(p.tgt + e);
+        if (g1 > ge + gs) is = __ldg(p.src + e);
       }
-      if (g0 < ge + gs && g1 > ge) it = __ldg(p.tgt + e);
-      if (g1 > ge + gs) is = __ldg(p.src + e);
-    }
-    const float* ea_row = p.ea + er * p.ld_ea;
-    const float* add_row = ai >= 0 ? p.ea_add + (long long)ai * p.ne : nullptr;
-    const float* t_row = p.node + (long long)it * p.ld_node - p.ne;
-    const float* s_row = p.node + (long long)is * p.ld_node - p.ne - p.ns;
-    float4 f[PER][2], ad[PER][2];
+      const float* ea_row = p.ea + er * p.ld_ea;
+      const float* add_row = ai >= 0 ? p.ea_add + (long long)ai * p.ne : nullptr;
+      const float* t_row = p.node + (long long)it * p.ld_node - p.ne;
+      const float* s_row = p.node + (long long)is * p.ld_node - p.ne - p.ns;
+      float4 f[PER][2], ad[PER][2];
 #pragma unroll
-    for (int u = 0; u < PER; ++u) {
-      const int g = g0 + u, k = g << 3;
-      f[u][0] = f[u][1] = ad[u][0] = ad[u][1] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (live && g < g1) {
-        const float* src = (g < ge) ? ea_row + k : (g < ge + gs ? t_row + k : s_row + k);
-        const float4* s4 = reinterpret_cast<const float4*>(src);
-        f[u][0] = __ldg(s4);
-        f[u][1] = __ldg(s4 + 1);
-        if (g < ge && add_row) {
-          const float4* a4 = reinterpret_cast<const float4*>(add_row + k);
-          ad[u][0] = __ldg(a4);
-          ad[u][1] = __ldg(a4 + 1);
+      for (int u = 0; u < PER; ++u) {
+        const int g = g0 + u, k = g << 3;
+        f[u][0] = f[u][1] = ad[u][0] = ad[u][1] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (live && g < g1) {
+          const float* src = (g < ge) ? ea_row + k : (g < ge + gs ? t_row + k : s_row + k);
+          const float4* s4 = reinterpret_cast<const float4*>(src);
+          f[u][0] = __ldg(s4);
+          f[u][1] = __ldg(s4 + 1);
+          if (g < ge && add_row) {
+            const float4* a4 = reinterpret_cast<const float4*>(add_row + k);
+            ad[u][0] = __ldg(a4);
+            ad[u][1] = __ldg(a4 + 1);
+          }
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < PER; ++u) {
+        const int g = g0 + u;
+        if (g < g1) {
+          f[u][0].x += ad[u][0].x; f[u][0].y += ad[u][0].y; f[u][0].z += ad[u][0].z; f[u][0].w += ad[u][0].w;
+          f[u][1].x += ad[u][1].x; f[u][1].y += ad[u][1].y; f[u][1].z += ad[u][1].z; f[u][1].w += ad[u][1].w;
+          uint4 hi, lo;
+          split8(reinterpret_cast<const float*>(&f[u][0]), hi, lo);
+          put_a8(sA, r, g << 3, hi);
+          put_a8(sA, r, Kp + (g << 3), lo);
         }
       }
     }
-#pragma unroll
-    for (int u = 0; u < PER; ++u) {
-      const int g = g0 + u;
-      if (g < g1) {
-        f[u][0].x += ad[u][0].x; f[u][0].y += ad[u][0].y; f[u][0].z += ad[u][0].z; f[u][0].w += ad[u][0].w;
-        f[u][1].x += ad[u][1].x; f[u][1].y += ad[u][1].y; f[u][1].z += ad[u][1].z; f[u][1].w += ad[u][1].w;
-        uint4 hi, lo;
-        split8(reinterpret_cast<const float*>(&f[u][0]), hi, lo);
-        put_a8(sA, r, g << 3, hi);
-        put_a8(sA, r, Kp + (g << 3), lo);
-      }
-    }
   } else {
-    for (int idx = tid; idx < BM * Kin; idx += THREADS) {
+    for (int idx = t; idx < BM * Kin; idx += 128) {
       const int r = idx / Kin, k = idx - r * Kin;
       const long long e = e0 + r;
       float v = 0.f;
@@ -426,29 +501,29 @@ __device__ __forceinline__ void build_a0(const FusedParams& p, unsigned char* sA
 __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  unsigned char* sA = smem;                                      // MAX_KA x 8 KB
-  unsigned char* sB = smem + (size_t)MAX_KA * A_KB_BYTES;        // ring of B stages
-  float* sC = reinterpret_cast<float*>(sB + STAGES * STAGE_BYTES);    // [64][CLD] accumulator tile
-  float* sY = sC + BM * CLD;                                     // [2][9][64] spherical harmonics per consumer thread
-  float* sFlush = sY + 2 * 9 * BM;                               // [4 warps][48][33] scatter staging
-  float* sMtab = sFlush + 4 * 48 * FLUSH_LD;                     // [MAX_PATHS][48]
+  unsigned char* sA = smem;                                      // [2 warpgroups][MAX_KA x 8 KB]
+  unsigned char* sB = smem + 2 * (size_t)A_IMAGE_BYTES;          // ring of B stages
+  float* sBuf = reinterpret_cast<float*>(sB + STAGES * STAGE_BYTES);   // [2 warpgroups][WG_BUF]: z rows / scatter staging
+  float* sY = sBuf + 2 * WG_BUF;                                 // [2][64][9] edge_weight * spherical harmonics per edge
+  float* sMtab = sY + 2 * BM * 9;                                // [MAX_PATHS][48]
   int* sTiles = reinterpret_cast<int*>(sMtab + MAX_PATHS * MTAB);   // [MAX_TILES][8]
-  uint32_t* sOps = reinterpret_cast<uint32_t*>(sTiles + MAX_TILES * 8);   // [2][SCHED_WORDS] MMA schedules
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sOps + 2 * SCHED_WORDS);
-  uint64_t* full = bars;                 // B stage s has landed (TMA complete_tx)
-  uint64_t* cfull = bars + STAGES;       // C holds a weight tile (128 MMA threads arrive)
-  uint64_t* cempty = cfull + 1;          // the consumers have drained C (128 consumer threads arrive)
+  uint64_t* full = reinterpret_cast<uint64_t*>(sTiles + MAX_TILES * 8);   // B stage s has landed (TMA complete_tx)
+  unsigned long long* sDbg = reinterpret_cast<unsigned long long*>(full + STAGES);   // [2][2] debug clocks per warpgroup
+  uint32_t* sOps = reinterpret_cast<uint32_t*>(sDbg + 4);       // [2 warpgroups][W1', W2'][SCHED_WORDS] MMA schedules
+  uint32_t* sRel = sOps + 4 * SCHED_WORDS;                       // [STAGES] releases of each stage
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
   const int S1 = p.K1p >> 4, S2 = p.Hp >> 4;
   for (int i = tid; i < p.n_tiles * 8; i += THREADS) sTiles[i] = p.tiles[i];
   for (int i = tid; i < p.n_paths * MTAB; i += THREADS) sMtab[i] = p.mtab[i];
-  if (tid == 32) build_ops(sOps, S1, gmma_desc_lo(smem_u32(sA)));
-  if (tid == 64) build_ops(sOps + SCHED_WORDS, S2, gmma_desc_lo(smem_u32(sA)));
+  if (tid % 32 == 0 && tid < 128) {
+    const int wg = tid >> 6, which = (tid >> 5) & 1;
+    build_ops(sOps + (2 * wg + which) * SCHED_WORDS, which ? S2 : S1, gmma_desc_lo(smem_u32(sA + wg * A_IMAGE_BYTES)));
+  }
+  if (tid < STAGES) sRel[tid] = 0u;
+  if (tid < 4) sDbg[tid] = 0ull;
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) mbar_init(&full[s], 1);
-    mbar_init(cfull, 128);
-    mbar_init(cempty, 128);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -457,7 +532,7 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
   // the edge count may live on the device (neighbour lists built without a host round trip): p.n_edges is then its bound
   long long n_edges = p.n_edges;
   if (p.n_edges_dev) { const long long nd = __ldg(p.n_edges_dev); n_edges = nd < n_edges ? (nd < 0 ? 0 : nd) : n_edges; }
-  const long long n_mtiles = (n_edges + BM - 1) / BM;
+  const long long n_mtiles = (n_edges + CTA_EDGES - 1) / CTA_EDGES;
   const long long my_units = blockIdx.x < n_mtiles ? (n_mtiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
   // debug clocks: a span is counted by subtracting its start from the counter and adding its end (modulo 2^64), so no start
   // value is held in registers through the kernel
@@ -468,159 +543,133 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
     atomicAdd(p.dbg + 26, 0ull - g0);
   }
 
-  // Each warpgroup runs its own loop over the CTA's edge tiles, so that the state one of them carries from tile to tile is
-  // not held in registers through the other's work (together they would not fit in 255 registers).  Both loops meet at
-  // the same two block-wide barriers per edge tile, around the A0' image that all threads build.
-  if (__shfl_sync(0xffffffffu, tid >> 7, 0) == 0) {     // warp-uniform for the compiler
-    Stream st;
-    st.sB = sB; st.full = full; st.tiles = sTiles; st.n1 = n1;
-    st.per_unit = p.n_kb1 + p.n_tiles * p.n_kb;
-    st.len = (uint32_t)(my_units * st.per_unit);
-    // the ring runs ahead across edge tiles: the next tile's W1' blocks are requested while this one is contracted
-    if (tid == 0)
-      for (int i = 0; i < STAGES; ++i) st.issue(p, (uint32_t)i);
-    uint32_t mc = 0, cc = 0;
-    for (long long mt = blockIdx.x; mt < n_mtiles; mt += gridDim.x) {
-      __syncthreads();
-      if (p.dbg && tid == 0) atomicAdd(p.dbg + 11, 0ull - (unsigned long long)clock64());
-      build_a0(p, sA, mt, n_edges, tid);
-      __syncthreads();
-      // ===== MMA warpgroup: hidden layer, then every N tile.  Every product is issued MAX_N wide: the stage rows past a
-      // tile's width hold stale data whose columns are never read, and one width keeps both accumulator sets in
-      // registers.  The tile loop is unrolled by two so that the set each tile uses is known at compile time.
-      Acc d0, d1;
-      const uint32_t* ops2 = sOps + SCHED_WORDS;
-      mma_kblocks(d0, p, st, sOps, 0, p.n_kb1, false, mc, tid);
-      mma_drain(p, st, mc, tid);
-      wgmma_fence_regs(d0);
-      store_hidden(d0, p, sA, tid);
-      mma_kblocks(d0, p, st, ops2, 0, p.n_kb, false, mc, tid);
-      for (int tile = 0;; tile += 2) {     // the last tile drains the pipe on the path that leaves the loop
-        if (tile + 1 >= p.n_tiles) {
-          mma_drain(p, st, mc, tid);
-          store_weights(d0, sC, cfull, cempty, cc, tid);
-          break;
-        }
-        weight_tile_next(d0, d1, p, st, ops2, mc, sC, cfull, cempty, cc, tid);
-        if (tile + 2 >= p.n_tiles) {
-          mma_drain(p, st, mc, tid);
-          store_weights(d1, sC, cfull, cempty, cc, tid);
-          break;
-        }
-        weight_tile_next(d1, d0, p, st, ops2, mc, sC, cfull, cempty, cc, tid);
-      }
-      if (p.dbg && tid == 0) { atomicAdd(p.dbg + 11, (unsigned long long)clock64()); atomicAdd(p.dbg + 12, 1ull); }
+  Stream st;
+  st.sB = sB; st.full = full; st.rel = sRel; st.tiles = sTiles; st.n1 = n1;
+  st.per_unit = p.n_kb1 + p.n_tiles * p.n_kb;
+  st.len = (uint32_t)(my_units * st.per_unit);
+  // the ring runs ahead across edge tiles: the next tile's W1' blocks are requested while this one is contracted
+  if (tid == 0)
+    for (int i = 0; i < STAGES; ++i) st.issue(p, (uint32_t)i);
+
+  // Warpgroup g owns edges 64 g .. 64 g + 63 of every 128-edge tile and does all of their work; the two warpgroups meet
+  // only at the stages of the shared B stream.
+  const int g = __shfl_sync(0xffffffffu, tid >> 7, 0);          // warp-uniform for the compiler
+  const int t = tid & 127, w4 = t >> 5, lane = tid & 31, q = lane & 3, bar = BAR_WG + g;
+  const int r0 = 16 * w4 + (lane >> 2);                          // this thread's accumulator rows (edges) r0, r0 + 8
+  const int rb = r0 + 8 * (q >> 1), ub = 8 * (q & 1);            // its z rows: edge rb, tile rows ub .. ub + 7
+  unsigned char* sAg = sA + (size_t)g * A_IMAGE_BYTES;
+  float* buf = sBuf + g * WG_BUF;
+  float* zrow = buf + rb * ZLD;
+  const float* zcon = buf + r0 * ZLD;
+  unsigned long long* dwait = (p.dbg && t == 0) ? sDbg + 2 * g : nullptr;
+  const uint32_t* ops1 = sOps + 2 * g * SCHED_WORDS;
+  const uint32_t* ops2 = ops1 + SCHED_WORDS;
+  uint32_t mc = 0;
+  for (long long mt = blockIdx.x; mt < n_mtiles; mt += gridDim.x) {
+    const long long e0 = mt * CTA_EDGES + g * BM;
+    if (p.dbg && tid == 0) atomicAdd(p.dbg + 11, 0ull - (unsigned long long)clock64());
+    build_a0(p, sAg, e0, n_edges, t);
+    named_bar(bar, 128);
+    // this thread's z edge: its source node's values, edge weight and spherical harmonics (component normalisation, e3nn
+    // polynomials); rows past the end see zero node values and scatter nothing
+    const long long eb = e0 + rb;
+    const bool vb = eb < n_edges;
+    const int src_b = vb ? __ldg(p.src + eb) : 0;
+    const long long erb = (vb && p.perm) ? (long long)__ldg(p.perm + eb) : eb;
+    const float ew_b = (vb && p.ew) ? __ldg(p.ew + erb) : 1.f;
+    float* Y = sY + (g * BM + rb) * 9;
+    if (ub == 0) {
+      float vx = vb ? p.vec_sign * __ldg(p.vec + 3 * erb) : 1.f, vy = vb ? p.vec_sign * __ldg(p.vec + 3 * erb + 1) : 0.f,
+            vz = vb ? p.vec_sign * __ldg(p.vec + 3 * erb + 2) : 0.f;
+      const float nrm = fmaxf(sqrtf(vx * vx + vy * vy + vz * vz), 1e-12f);
+      vx /= nrm; vy /= nrm; vz /= nrm;
+      const float s3 = 1.7320508075688772f, s5 = 2.23606797749979f, s15 = 3.872983346207417f;
+      Y[0] = ew_b;
+      Y[1] = ew_b * (s3 * vx); Y[2] = ew_b * (s3 * vy); Y[3] = ew_b * (s3 * vz);
+      Y[4] = ew_b * (s15 * vx * vz);
+      Y[5] = ew_b * (s15 * vx * vy);
+      Y[6] = ew_b * (s5 * (vy * vy - 0.5f * (vx * vx + vz * vz)));
+      Y[7] = ew_b * (s15 * vy * vz);
+      Y[8] = ew_b * (0.5f * s15 * (vz * vz - vx * vx));
     }
-  } else {
-    uint32_t cc_con = 0;
-    for (long long mt = blockIdx.x; mt < n_mtiles; mt += gridDim.x) {
-      __syncthreads();
-      build_a0(p, sA, mt, n_edges, tid);
-      __syncthreads();
-      // ===== consumers: two threads per edge (warps q and q ^ 2), each contracting alternate 32-column chunks ========
-      const int q = warp & 3, half = q >> 1, ct = (q & 1) * 32 + lane;     // ct = row of the edge tile
-      const long long e = mt * BM + ct;
-      const bool valid = e < n_edges;
-      const int src_e = valid ? __ldg(p.src + e) : 0, dst_e = valid ? __ldg(p.tgt + e) : -1;
-      const long long er = (valid && p.perm) ? (long long)__ldg(p.perm + e) : e;
-      const float ew_e = (valid && p.ew) ? __ldg(p.ew + er) : 1.f;
-      // runs of equal scatter targets inside the warp (rows past the end form their own, never flushed, runs)
-      const int key_up = __shfl_up_sync(0xffffffffu, dst_e, 1);
-      const uint32_t head_mask = __ballot_sync(0xffffffffu, lane == 0 || key_up != dst_e || !valid);
-      float* sF = sFlush + q * 48 * FLUSH_LD;
-      const float* sFp = sFlush + (q ^ 2) * 48 * FLUSH_LD;     // the partner warp's partial sums
-      float* sYh = sY + half * 9 * BM;
-      {   // real spherical harmonics of the edge vector, component normalisation (e3nn polynomials)
-        float vx = valid ? p.vec_sign * __ldg(p.vec + 3 * er) : 1.f, vy = valid ? p.vec_sign * __ldg(p.vec + 3 * er + 1) : 0.f,
-              vz = valid ? p.vec_sign * __ldg(p.vec + 3 * er + 2) : 0.f;
-        const float nrm = fmaxf(sqrtf(vx * vx + vy * vy + vz * vz), 1e-12f);
-        vx /= nrm; vy /= nrm; vz /= nrm;
-        const float s3 = 1.7320508075688772f, s5 = 2.23606797749979f, s15 = 3.872983346207417f;
-        sYh[0 * BM + ct] = 1.f;
-        sYh[1 * BM + ct] = s3 * vx; sYh[2 * BM + ct] = s3 * vy; sYh[3 * BM + ct] = s3 * vz;
-        sYh[4 * BM + ct] = s15 * vx * vz;
-        sYh[5 * BM + ct] = s15 * vx * vy;
-        sYh[6 * BM + ct] = s5 * (vy * vy - 0.5f * (vx * vx + vz * vz));
-        sYh[7 * BM + ct] = s15 * vy * vz;
-        sYh[8 * BM + ct] = 0.5f * s15 * (vz * vz - vx * vx);
+    __syncwarp();
+    // this lane's scatter edge: runs of equal targets inside the warp (rows past the end form their own, never flushed, runs)
+    const long long es = e0 + 32 * (w4 & 1) + lane;
+    const bool vs = es < n_edges;
+    const int dst_s = vs ? __ldg(p.tgt + es) : -1;
+    const int key_up = __shfl_up_sync(0xffffffffu, dst_s, 1);
+    const uint32_t head_mask = __ballot_sync(0xffffffffu, lane == 0 || key_up != dst_s || !vs);
+
+    const float* xrow = p.x + (long long)src_b * p.ld_x;
+    float xn[XN], M[9], acc[NACC_MAX];
+    prefetch_tile(xrow, sTiles, ub, p.x_vec2, xn);
+    Acc d;
+    mma_product(d, p, st, ops1, p.n_kb1, mc, bar, t, dwait);
+    store_hidden(d, p, sAg, t, bar);
+    for (int ti = 0; ti < p.n_tiles; ++ti) {
+      const int* tt = sTiles + ti * 8;
+      const int kind = tt[0], d_in = tt[4], out_off = tt[5], flags = tt[6];
+      if (flags & 1) {
+#pragma unroll
+        for (int i = 0; i < NACC_MAX; ++i) acc[i] = 0.f;
       }
-      const float* xrow = p.x + (long long)src_e * p.ld_x;
-      const float* crow = sC + ct * CLD;
-      float acc[48], xn[XN], M[9];
-      prefetch_x(xrow + sTiles[2], sTiles[3] * sTiles[4], p.x_vec2, xn);
-      for (int t = 0; t < p.n_tiles; ++t, ++cc_con) {
-        const int* ti = sTiles + t * 8;
-        const int kind = ti[0], d_in = ti[4], out_off = ti[5], flags = ti[6];
-        const int tn = (t + 1 < p.n_tiles) ? t + 1 : t;          // next tile (the last one requests nothing)
-        const float* xnext = xrow + sTiles[tn * 8 + 2];
-        const int cnt_next = (t + 1 < p.n_tiles) ? sTiles[tn * 8 + 3] * sTiles[tn * 8 + 4] : 0;
-        if (flags & 1) {
+      // M[i,k] = edge_weight * sum_j coef*C[i,j,k] * Y[sh_off + j]  (at most 3x3 for the supported paths; row-major,
+      // stride 3), rebuilt only when the tile belongs to another path than its predecessor: dense table, fully unrolled
+      if (flags & 4) {
+        const float* T = sMtab + tt[7] * MTAB;
+        const int sh_off = (flags >> 8) & 0xff;
+        float yb[5];
 #pragma unroll
-          for (int i = 0; i < 48; ++i) acc[i] = 0.f;
+        for (int j = 0; j < 5; ++j) yb[j] = Y[min(sh_off + j, 8)];
+#pragma unroll
+        for (int ik = 0; ik < 9; ++ik) {
+          float a = 0.f;
+#pragma unroll
+          for (int j = 0; j < 5; ++j) a = fmaf(T[ik * 5 + j], yb[j], a);
+          M[ik] = a;
         }
-        // M[i,k] = edge_weight * sum_j coef*C[i,j,k] * Y[sh_off + j]  (at most 3x3 for the supported paths; row-major,
-        // stride 3), rebuilt only when the tile belongs to another path than its predecessor: dense table, fully unrolled
-        if (flags & 4) {
-          const float* T = sMtab + ti[7] * MTAB;
-          const int sh_off = (flags >> 8) & 0xff;
-          float yb[5];
-#pragma unroll
-          for (int j = 0; j < 5; ++j) yb[j] = sYh[min(sh_off + j, 8) * BM + ct];
-#pragma unroll
-          for (int ik = 0; ik < 9; ++ik) {
-            float a = 0.f;
-#pragma unroll
-            for (int j = 0; j < 5; ++j) a = fmaf(T[ik * 5 + j], yb[j], a);
-            M[ik] = a * ew_e;
-          }
-        }
-        const uint32_t par = cc_con & 1;
-        const int nch = ti[1] >> 5;
+      }
+      // z of this tile from the node values prefetched one tile ahead; then the next tile's values are requested, so that
+      // their latency hides behind this tile's MMAs
+      __syncwarp();                              // the quad has read the previous tile's z rows
+      switch (kind) {
+        case 0: build_z<1, 4>(xn, d_in, M, zrow, ub); break;
+        case 1: build_z<3, 16>(xn, d_in, M, zrow, ub); break;
+        case 2: build_z<1, 8>(xn, d_in, M, zrow, ub); break;
+        default: build_z<3, 16>(xn, d_in, M, zrow, ub); break;
+      }
+      __syncwarp();
+      if (ti + 1 < p.n_tiles) prefetch_tile(xrow, tt + 8, ub, p.x_vec2, xn);
+      mma_product(d, p, st, ops2, p.n_kb, mc, bar, t, dwait);
+      const long long c0 = dwait ? clock64() : 0;
+      const int nch = tt[1] >> 5;
+      switch (kind) {
+        case 0: contract<48, 1, 4>(d, zcon, nch, q, acc); break;
+        case 1: contract<10, 3, 16>(d, zcon, nch, q, acc); break;
+        case 2: contract<16, 1, 8>(d, zcon, nch, q, acc); break;
+        default: contract<4, 3, 16>(d, zcon, nch, q, acc); break;
+      }
+      if (flags & 2) {
         switch (kind) {
-          case 0: tile_body<48, 1, 4>(crow, nch, half, xn, d_in, M, acc, cfull, par); break;
-          case 1: tile_body<10, 3, 16>(crow, nch, half, xn, d_in, M, acc, cfull, par); break;
-          case 2: tile_body<16, 1, 8>(crow, nch, half, xn, d_in, M, acc, cfull, par); break;
-          default: tile_body<4, 3, 16>(crow, nch, half, xn, d_in, M, acc, cfull, par); break;
-        }
-        mbar_arrive(cempty);
-        // the next tile's node values are requested only now, so that they are not held in registers through the
-        // contraction; their latency overlaps the scatter and the wait for the next accumulator tile
-        prefetch_x(xnext, cnt_next, p.x_vec2, xn);
-        if (flags & 2) {
-          // end of an output irrep: scatter-add.  Both warps of the pair stage their 32 x nacc partial results in shared
-          // memory (padded rows: conflict-free both ways); lane i of warp `half` then walks the 32 edges adding the two
-          // partial sums, sums runs of equal targets (CSR order makes them contiguous; unsorted input just yields runs of
-          // length one) and issues ONE fully coalesced RED.ADD per run for output value 32 half + i.
-          const int nacc = (kind == 0) ? 48 : (kind == 1 ? 30 : (kind == 2 ? 16 : 12));
-#pragma unroll
-          for (int i = 0; i < 48; ++i)
-            if (i < nacc) sF[i * FLUSH_LD + lane] = acc[i];
-          named_bar(BAR_PAIR + (q & 1), 64);
-          const int i = 32 * half + lane;
-          if (32 * half < nacc) {
-            const bool act = i < nacc;
-            const float* col = sF + (act ? i : 0) * FLUSH_LD;
-            const float* colp = sFp + (act ? i : 0) * FLUSH_LD;
-            float s = 0.f;
-#pragma unroll
-            for (int le = 0; le < 32; ++le) {
-              s += col[le] + colp[le];
-              if (le == 31 || ((head_mask >> (le + 1)) & 1)) {          // warp-uniform: last edge of a run
-                const int d = __shfl_sync(0xffffffffu, dst_e, le);
-                if (d >= 0 && act) atomicAdd(p.sum + (long long)d * p.d_out + out_off + i, s);
-                s = 0.f;
-              }
-            }
-          }
-          named_bar(BAR_PAIR + (q & 1), 64);
+          case 0: flush<48, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+          case 1: flush<10, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+          case 2: flush<16, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+          default: flush<4, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
         }
       }
-      if (p.cnt && half == 0) {       // edge counts per target: one atomic per run, issued by the run's first lane
-        const bool head = (head_mask >> lane) & 1;
-        const uint32_t above = (lane == 31) ? 0u : (head_mask >> (lane + 1));
-        const int run_len = above ? __ffs(above) : 32 - lane;
-        if (head && valid) atomicAdd(p.cnt + dst_e, (float)run_len);
-      }
+      if (dwait) dwait[1] += (unsigned long long)(clock64() - c0);
+    }
+    if (p.cnt && w4 < 2) {         // edge counts per target: one atomic per run, issued by the run's first lane
+      const bool head = (head_mask >> lane) & 1;
+      const uint32_t above = (lane == 31) ? 0u : (head_mask >> (lane + 1));
+      const int run_len = above ? __ffs(above) : 32 - lane;
+      if (head && vs) red_add(p.cnt + dst_s, (float)run_len);
+    }
+    if (p.dbg && tid == 0) { atomicAdd(p.dbg + 11, (unsigned long long)clock64()); atomicAdd(p.dbg + 12, 2ull); }
+    if (dwait) {
+      atomicAdd(p.dbg + 13, dwait[0]);
+      atomicAdd(p.dbg + 14, dwait[1]);
+      dwait[0] = dwait[1] = 0ull;
     }
   }
   if (p.dbg && blockIdx.x == 0 && tid == 0) {
@@ -655,8 +704,10 @@ unsigned long long* fused_debug_buffer(int dev) {
 }  // namespace
 
 // Diagnostics (DDB200_FUSED_DEBUG=1 only): copies the 32 clock counters of the fused kernel (current device) to `out` and
-// clears them.  [11] clocks spent per edge tile (summed over tiles), [12] edge tiles, [25] / [26] clock64 ticks / ns of
-// CTA 0 over the launch.  Synchronises the device.
+// clears them.  [11] clocks spent per 128-edge tile by warpgroup 0 (summed over tiles), [12] 64-edge units (two per
+// 128-edge tile), [13] clocks the warpgroups spent waiting for a B stage to land, [14] clocks they spent contracting and
+// scattering (both summed over the two warpgroups), [25] / [26] clock64 ticks / ns of CTA 0 over the launch.  Synchronises
+// the device.
 extern "C" int ddb200_fused_debug_read(uint64_t* out) {
   int dev = 0;
   cudaGetDevice(&dev);
@@ -703,10 +754,10 @@ extern "C" int ddb200_fused_conv(const ddb200_fused_args* a, void* stream) {
   if (dev < 0 || dev >= MAX_DEVICES) return DDB200_EINVAL;
   p.dbg = fused_debug_buffer(dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long n_mtiles = (a->n_edges + BM - 1) / BM;
-  const size_t fixed = (BM * CLD + 2 * 9 * BM + 4 * 48 * FLUSH_LD + MAX_PATHS * MTAB) * 4 + MAX_TILES * 8 * 4 +
-                       2 * SCHED_WORDS * 4 + (STAGES + 2) * sizeof(uint64_t) + 1024;
-  const size_t smem = (size_t)MAX_KA * A_KB_BYTES + (size_t)STAGES * STAGE_BYTES + fixed;
+  const long long n_mtiles = (a->n_edges + CTA_EDGES - 1) / CTA_EDGES;
+  const size_t fixed = (2 * WG_BUF + 2 * BM * 9 + MAX_PATHS * MTAB) * 4 + MAX_TILES * 8 * 4 + (STAGES + 4) * sizeof(uint64_t) +
+                       (4 * SCHED_WORDS + STAGES) * 4 + 1024;
+  const size_t smem = 2 * (size_t)A_IMAGE_BYTES + (size_t)STAGES * STAGE_BYTES + fixed;
   if (smem > 227 * 1024) return DDB200_ESMEM;
   if (!g_dev[dev].attr_done) {      // the opt-in is a per-device attribute
     const cudaError_t e = cudaFuncSetAttribute(fused_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -64,7 +64,8 @@ def scan():
 
 def layer(li, E, N, deg):
     """Time the fused kernel on layer li's table (E edges, N nodes, `deg` edges per target); with DDB200_FUSED_DEBUG=1 also
-    the clocks per 64-edge tile against the tensor-pipe ideal and the rate at which the operand images stream from L2."""
+    the clocks per 64 edges against the tensor-pipe ideal, the rate at which the operand images stream from L2, and where
+    a warpgroup's time goes: waiting for weight stages to land, and contracting + scattering."""
     from diffdock_b200 import _lib, fused
     from diffdock_b200.tensor_layers import get_irrep_seq
     from diffdock_b200.tp_table import build_table
@@ -103,20 +104,27 @@ def layer(li, E, N, deg):
     flops = ((E + 63) // 64) * plan.mma_flops_per_tile
     r = {'layer': li, 'E': E, 'tiles': plan.n_tiles, 'ms': round(ms, 3), 'bf16_issued_TFLOPs': round(flops / ms / 1e9, 1)}
     if have_dbg and _lib.lib().ddb200_fused_debug_read(dbg) == 0:
-        units = max(int(dbg[12]), 1)
-        clk = int(dbg[11]) / units
+        units = max(int(dbg[12]), 1)                  # 64-edge units: two per 128-edge CTA tile, one per warpgroup
+        clk = int(dbg[11]) / units                     # CTA clocks per 64 edges
         s = 3 * ((H + 15) // 16) + 1                  # MMA steps per product (hidden layer and weight tiles alike here)
         r['clk_per_edge_tile'] = int(clk)
         # 4096 bf16 FLOP / clk / SM (H100 data sheet): one 64x192x16 MMA = 96 clocks
         r['ideal_clk_per_edge_tile'] = 96 * s * (plan.n_tiles + 1)
         r['frac_of_ideal'] = round(r['ideal_clk_per_edge_tile'] / clk, 3)
-        # operand-image bytes streamed per edge tile, as the kernel's TMA ring fetches them: the rows a product reads (W1': the
-        # padded hidden width; W2': each tile's MMA width) x 128 B per k-block
+        # operand-image bytes streamed per 128-edge tile (one stream per CTA, read by both warpgroups), as the kernel's TMA
+        # ring fetches them: the rows a product reads (W1': the padded hidden width; W2': each tile's MMA width) x 128 B per
+        # k-block
         hp, k1p = (H + 15) // 16 * 16, (K1 + 15) // 16 * 16
         n_kb, n_kb1 = (2 * hp + 16 + 63) // 64, (2 * k1p + 16 + 63) // 64
         img_bytes = 128 * (n_kb1 * hp + n_kb * int(plan.tiles[:, 1].sum()))
-        r['image_B_per_clk_per_sm'] = round(img_bytes / clk, 1)
-        r['edge_tiles'] = units // 5
+        r['image_B_per_clk_per_sm'] = round(img_bytes / (2 * clk), 1)
+        # a warpgroup spends 2 clk on its 64 edges; the share of it spent waiting for a stage to land and contracting
+        wg_clk = 2 * clk
+        r['stage_wait_clk_per_64'] = int(dbg[13] / units)
+        r['contract_clk_per_64'] = int(dbg[14] / units)
+        r['stage_wait_frac'] = round(dbg[13] / units / wg_clk, 3)
+        r['contract_frac'] = round(dbg[14] / units / wg_clk, 3)
+        r['edge_units_64'] = units // 5
         r['sm_clock_ghz_in_kernel'] = round(dbg[25] / max(dbg[26], 1), 3)     # clock64 ticks per globaltimer ns, CTA 0
     del x, tgt, src, vec, ea, out, cnt
     return r
