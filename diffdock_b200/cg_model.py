@@ -434,20 +434,29 @@ class CGModel(nn.Module):
         cnt = ops.radius_count(xpos, pos, x_ptr, c['lig_batch32'], r=r, r_per_graph=rpg, max_num_neighbors=10000)
         incl = torch.cumsum(cnt, 0, dtype=torch.int32)
         n_dev = incl[-1:]
-        slot = torch.empty((n_lig, max(x_max, 1)), dtype=torch.int32, device=pos.device)
+        # the reverse search below has no cap and reads each pair's forward position from slot[ligand atom, x], so it is
+        # only right while the forward cap cannot bind; past that the reverse list is the forward one sorted by x
+        slot = torch.empty((n_lig, max(x_max, 1)), dtype=torch.int32, device=pos.device) if x_max <= 10000 else None
         # rows beyond the live count must be valid (zero) when library ops gather over the whole buffer: the smooth edge
         # weight, or the embedding MLP when its shape is outside the edge-embedding kernel's templates
         padded_valid = self.smooth_edges or not self._edge_embed_in_kernel(mlp, gs)
         f_tgt, f_src, vec, _, _ = ops.graph_fill(
             xpos, pos, x_ptr, c['lig_batch32'], (incl - cnt).contiguous(), cap, r=r, r_per_graph=rpg,
-            max_num_neighbors=10000, slot_out=slot, slot_ld=slot.shape[1], col_offset=col_off,
+            max_num_neighbors=10000, slot_out=slot, slot_ld=slot.shape[1] if slot is not None else 0, col_offset=col_off,
             fill_row=0 if padded_valid else None)
-        cnt_r = ops.radius_count(pos, xpos, c['lig_ptr'], x_batch32, r=r, r_per_graph=rpg, max_num_neighbors=1 << 30)
-        incl_r = torch.cumsum(cnt_r, 0, dtype=torch.int32)
-        b_tgt, b_src, _, _, perm = ops.graph_fill(
-            pos, xpos, c['lig_ptr'], x_batch32, (incl_r - cnt_r).contiguous(), cap, r=r, r_per_graph=rpg,
-            max_num_neighbors=1 << 30, want_vec=False, slot_in=slot, y_ptr=x_ptr, slot_ld=slot.shape[1], want_perm=True,
-            row_offset=col_off)
+        if slot is not None:
+            cnt_r = ops.radius_count(pos, xpos, c['lig_ptr'], x_batch32, r=r, r_per_graph=rpg, max_num_neighbors=1 << 30)
+            incl_r = torch.cumsum(cnt_r, 0, dtype=torch.int32)
+            b_tgt, b_src, _, _, perm = ops.graph_fill(
+                pos, xpos, c['lig_ptr'], x_batch32, (incl_r - cnt_r).contiguous(), cap, r=r, r_per_graph=rpg,
+                max_num_neighbors=1 << 30, want_vec=False, slot_in=slot, y_ptr=x_ptr, slot_ld=slot.shape[1], want_perm=True,
+                row_offset=col_off)
+        else:
+            # stable sort by the x end; rows past the live count get a key above every x, so they sort last
+            n_rows = col_off + xpos.shape[0]
+            live = torch.arange(f_src.shape[0], dtype=torch.int32, device=pos.device) < n_dev
+            b_tgt, perm, _ = ops.csr_sort_by_target(torch.where(live, f_src, n_rows), n_rows + 1)
+            b_src, perm = f_tgt[perm], perm.int()
         ea = self._cross_edge_embedding(lig.node_sigma_emb, vec, f_tgt, n_dev, mlp, gs)
         ew = None
         if self.smooth_edges:

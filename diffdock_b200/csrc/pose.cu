@@ -239,11 +239,19 @@ __global__ void pose_update_kernel(const float* pos, int n_atoms, int n_bonds,
       v1[c] = H[0][c] * u1[0] + H[1][c] * u1[1] + H[2][c] * u1[2];
       v2[c] = H[0][c] * u2[0] + H[1][c] * u2[1] + H[2][c] * u2[2];
     }
-    double n1 = sqrt(v1[0] * v1[0] + v1[1] * v1[1] + v1[2] * v1[2]);
-    for (int c = 0; c < 3; ++c) v1[c] /= n1;
+    // H of rank < 2 (every atom on one line, e.g. a linear ligand whose torsions cannot move an atom off it): v2 is then
+    // arbitrary in the plane orthogonal to v1, and any choice gives a rotation about that line, which moves no atom
+    const double n1 = sqrt(v1[0] * v1[0] + v1[1] * v1[1] + v1[2] * v1[2]);
+    for (int c = 0; c < 3; ++c) v1[c] = n1 > 0 ? v1[c] / n1 : u1[c];     // n1 = 0: H = 0, every atom at the centroid
     double d12 = v1[0] * v2[0] + v1[1] * v2[1] + v1[2] * v2[2];
     for (int c = 0; c < 3; ++c) v2[c] -= d12 * v1[c];
     double n2 = sqrt(v2[0] * v2[0] + v2[1] * v2[1] + v2[2] * v2[2]);
+    if (!(n2 > 1e-10 * n1)) {        // complete the frame with the coordinate axis least aligned with v1
+      int k = fabs(v1[0]) <= fabs(v1[1]) ? 0 : 1;
+      if (fabs(v1[2]) < fabs(v1[k])) k = 2;
+      for (int c = 0; c < 3; ++c) v2[c] = (c == k) - v1[k] * v1[c];
+      n2 = sqrt(v2[0] * v2[0] + v2[1] * v2[1] + v2[2] * v2[2]);
+    }
     for (int c = 0; c < 3; ++c) v2[c] /= n2;
     const double u3[3] = {u1[1] * u2[2] - u1[2] * u2[1], u1[2] * u2[0] - u1[0] * u2[2], u1[0] * u2[1] - u1[1] * u2[0]};
     const double v3[3] = {v1[1] * v2[2] - v1[2] * v2[1], v1[2] * v2[0] - v1[0] * v2[2], v1[0] * v2[1] - v1[1] * v2[0]};
