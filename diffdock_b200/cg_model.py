@@ -21,7 +21,7 @@ from torch import nn
 from . import ops
 from .irreps import irreps_str, sh_irreps
 from .layers import (AtomEncoder, GaussianSmearing, _mlp, check_forward, cross_cutoff, cross_graph, edge_cutoff, edge_weight,
-                     ligand_graph)
+                     ligand_graph, score_heads)
 from .synthetic import LIG_FEATURE_DIMS as lig_feature_dims, REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims
 from .tensor_layers import TensorProductConvLayer, get_irrep_seq
 from .tp_table import full_tensor_product
@@ -46,26 +46,6 @@ def _rr_joint(c, n_lig):
     if n_lig not in c.setdefault('rr_tgt32', {}):
         c['rr_tgt32'][n_lig] = (_i32(c['rr_tgt'] + n_lig), _i32(c['rr_src'] + n_lig))
     return c['rr_tgt32'][n_lig]
-
-
-def _sh_l2(vec):
-    """Component-normalised l=2 real spherical harmonics of the normalised vectors (o3.spherical_harmonics("2e", ...),
-    models/cg_model.py:411)."""
-    v = torch.nn.functional.normalize(vec, dim=-1)
-    x, y, z = v[:, 0], v[:, 1], v[:, 2]
-    s5, s15 = math.sqrt(5.0), math.sqrt(15.0)
-    return torch.stack([s15 * x * z, s15 * x * y, s5 * (y * y - 0.5 * (x * x + z * z)), s15 * y * z,
-                        0.5 * s15 * (z * z - x * x)], dim=-1)
-
-
-def _sh_full(vec, lmax):
-    v = torch.nn.functional.normalize(vec, dim=-1)
-    cols = [torch.ones_like(v[:, :1])]
-    if lmax >= 1:
-        cols.append(math.sqrt(3.0) * v)
-    if lmax >= 2:
-        cols.append(_sh_l2(vec))
-    return torch.cat(cols, dim=-1)
 
 
 class CGModel(nn.Module):
@@ -407,6 +387,16 @@ class CGModel(nn.Module):
         """Bonds + radius graph, CSR by target, built on the device (models/cg_model.py:467-497), and the ligand embedding
         layers over it: ``(ligand node features, edge group)``."""
         lig = data['ligand']
+        g = self._ligand_edges_sync_free(data, c)
+        node = self.lig_node_embedding(torch.cat([lig.x.float(), lig.node_sigma_emb], 1))
+        for layer in self.lig_emb_layers:
+            node = layer.forward_groups(node, [g], gather_scalars=self.ns)
+        return node, g
+
+    def _ligand_edges_sync_free(self, data, c):
+        """The edge group of the ligand graph (bonds + radius graph, CSR by target) in a capacity buffer; sets
+        ``node_sigma_emb`` on the ligand."""
+        lig = data['ligand']
         pos = lig.pos.float().contiguous()
         lig.node_sigma_emb = self.timestep_emb_func(lig.node_t['tr'])
         cnt = ops.radius_count(pos, pos, c['lig_ptr'], c['lig_batch32'], r=self.lig_max_radius, max_num_neighbors=33,
@@ -417,12 +407,8 @@ class CGModel(nn.Module):
             max_num_neighbors=33, exclude_self=True, pre_ptr=c['pre_ptr'], pre_col=c['pre_col'], want_eid=True, fill_row=0)
         attr = torch.cat([c['pre_attr'][eid.long()], lig.node_sigma_emb[tgt.long()],
                           self.lig_distance_expansion(vec.norm(dim=-1))], 1)
-        g = (tgt, src, self.lig_edge_embedding(attr), vec, _flat(self.get_edge_weight(vec, self.lig_max_radius)),
-             dict(n_edges_dev=incl[-1:]))
-        node = self.lig_node_embedding(torch.cat([lig.x.float(), lig.node_sigma_emb], 1))
-        for layer in self.lig_emb_layers:
-            node = layer.forward_groups(node, [g], gather_scalars=self.ns)
-        return node, g
+        return (tgt, src, self.lig_edge_embedding(attr), vec, _flat(self.get_edge_weight(vec, self.lig_max_radius)),
+                dict(n_edges_dev=incl[-1:]))
 
     def _cross_graph_sync_free(self, data, c, xpos, x_ptr, x_batch32, x_max, cap, r, rpg, col_off, mlp, gs, vec_sign):
         """Ligand <- x edges (x: residues or receptor atoms at ``xpos``, numbered from ``col_off`` in the joint graph) in a
@@ -548,64 +534,4 @@ class CGModel(nn.Module):
         return self._heads(data, c, node[:n_lig], tr_sigma, rot_sigma, tor_sigma, sync_free=False)
 
     def _heads(self, data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_free):
-        lig = data['ligand']
-        ns, B = self.ns, data.num_graphs
-        n_lig = lig_node.shape[0]
-        # -- translation / rotation head (:368-395) -----------------------------------------------------------------
-        pos = lig.pos.float()
-        arange = torch.arange(n_lig, device=pos.device)
-        center = torch.zeros((B, 3), device=pos.device).index_add_(0, lig.batch, pos)
-        center = center / c['lig_cnt_f']
-        c_vec = pos - center[lig.batch]
-        c_ea = torch.cat([self.center_distance_expansion(c_vec.norm(dim=-1)), lig.node_sigma_emb], 1)
-        c_ea = self.center_edge_embedding(c_ea)
-        idx = arange if self.fixed_center_conv else lig.batch            # hazard C.6: graph id indexes lig_node
-        c_ea = torch.cat([c_ea, lig_node[idx, :ns]], -1)
-        glob = self.final_conv(lig_node, torch.stack([lig.batch, arange]), c_ea, None, out_nodes=B, edge_vec=c_vec,
-                               assume_sorted=True)
-        tr_pred = glob[:, :3] + (glob[:, 6:9] if not self.odd_parity else 0)
-        rot_pred = glob[:, 3:6] + (glob[:, 9:] if not self.odd_parity else 0)
-        data.graph_sigma_emb = self.timestep_emb_func(data.complex_t['tr'])
-        tr_norm = torch.linalg.vector_norm(tr_pred, dim=1).unsqueeze(1)
-        tr_pred = tr_pred / tr_norm * self.tr_final_layer(torch.cat([tr_norm, data.graph_sigma_emb], dim=1))
-        rot_norm = torch.linalg.vector_norm(rot_pred, dim=1).unsqueeze(1)
-        rot_pred = rot_pred / rot_norm * self.rot_final_layer(torch.cat([rot_norm, data.graph_sigma_emb], dim=1))
-        if self.scale_by_sigma:
-            tr_pred = tr_pred / tr_sigma.unsqueeze(1)
-            rot_pred = rot_pred * self._so3_score_norm(rot_sigma).unsqueeze(1)
-
-        if self.no_torsion or c['n_bonds'] == 0:
-            return tr_pred, rot_pred, torch.empty(0, device=self.device), None
-
-        # -- torsion head (:406-423) --------------------------------------------------------------------------------
-        bonds = c['bonds']
-        n_bonds = c['n_bonds']
-        bond_pos = ((pos[bonds[0]] + pos[bonds[1]]) / 2).contiguous()
-        if sync_free:
-            # upper-bound buffer (32 atoms per bond, models/cg_model.py:630); slots beyond the live count point at an extra
-            # dummy bond row (index n_bonds) that is dropped after the convolution
-            pos_c = pos.contiguous()
-            cnt = ops.radius_count(pos_c, bond_pos, c['lig_ptr'], c['bond_batch32'], r=self.lig_max_radius, max_num_neighbors=32)
-            incl = torch.cumsum(cnt, 0, dtype=torch.int32)
-            bi32, ai32, t_vec, _, _ = ops.graph_fill(pos_c, bond_pos, c['lig_ptr'], c['bond_batch32'], (incl - cnt).contiguous(),
-                                                     c['cap_tor'], r=self.lig_max_radius, max_num_neighbors=32, fill_row=n_bonds)
-            bi, ai = bi32.long(), ai32.long()
-            bi_g = bi.clamp_max(n_bonds - 1)            # gathers of per-bond quantities for the dummy slots: any valid row
-            n_out = n_bonds + 1
-        else:
-            bi, ai, _ = ops.radius(pos, bond_pos, c['lig_ptr'], c['bond_batch'], r=self.lig_max_radius, max_num_neighbors=32)
-            bi, ai = bi.long(), ai.long()
-            t_vec = pos[ai] - bond_pos[bi]
-            bi_g, n_out = bi, n_bonds
-        t_ea = self.final_edge_embedding(self.lig_distance_expansion(t_vec.norm(dim=-1)))
-        bond_vec = pos[bonds[1]] - pos[bonds[0]]
-        bond_attr = lig_node[bonds[0]] + lig_node[bonds[1]]
-        t_sh = torch.einsum('ea,eb,abc->ec', _sh_full(t_vec, self.sh_lmax), _sh_l2(bond_vec)[bi_g], self._tor_tp)
-        t_ea = torch.cat([t_ea, lig_node[ai, :ns], bond_attr[bi_g, :ns]], -1)
-        tor_pred = self.tor_bond_conv(lig_node, torch.stack([bi, ai]), t_ea, t_sh, out_nodes=n_out, reduce='mean',
-                                      edge_weight=self.get_edge_weight(t_vec, self.lig_max_radius), assume_sorted=True)
-        tor_pred = self.tor_final_layer(tor_pred[:n_bonds]).squeeze(1)
-        edge_sigma = tor_sigma[c['bond_lig_batch']]
-        if self.scale_by_sigma:
-            tor_pred = tor_pred * torch.sqrt(self._torus_score_norm(edge_sigma))
-        return tr_pred, rot_pred, tor_pred, None
+        return score_heads(self, data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_free) + (None,)

@@ -1,5 +1,7 @@
 """Embedding layers with the reference's parameter names (models/layers.py) - plain PyTorch modules on the device
 (small dense ops; the hot convolution lives in csrc/) - and the graph plumbing the four models share."""
+import math
+
 import numpy as np
 import torch
 from torch import nn
@@ -82,6 +84,93 @@ def confidence_head(model, data, lig_node):
     pooled = torch.zeros((B, scal.shape[1]), device=scal.device, dtype=scal.dtype).index_add_(0, batch, scal)
     pooled = pooled / torch.bincount(batch, minlength=B).clamp(min=1).unsqueeze(1)
     return model.confidence_predictor(pooled).squeeze(dim=-1)
+
+
+def _sh_l2(vec):
+    """Component-normalised l=2 real spherical harmonics of the normalised vectors (o3.spherical_harmonics("2e", ...),
+    models/cg_model.py:411)."""
+    v = torch.nn.functional.normalize(vec, dim=-1)
+    x, y, z = v[:, 0], v[:, 1], v[:, 2]
+    s5, s15 = math.sqrt(5.0), math.sqrt(15.0)
+    return torch.stack([s15 * x * z, s15 * x * y, s5 * (y * y - 0.5 * (x * x + z * z)), s15 * y * z,
+                        0.5 * s15 * (z * z - x * x)], dim=-1)
+
+
+def _sh_full(vec, lmax):
+    v = torch.nn.functional.normalize(vec, dim=-1)
+    cols = [torch.ones_like(v[:, :1])]
+    if lmax >= 1:
+        cols.append(math.sqrt(3.0) * v)
+    if lmax >= 2:
+        cols.append(_sh_l2(vec))
+    return torch.cat(cols, dim=-1)
+
+
+def score_heads(model, data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_free):
+    """The translation / rotation and torsion heads of the score models, ``(tr [B, 3], rot [B, 3], tor [n_bonds])``
+    (models/cg_model.py:368-424 = models/aa_model.py:443-508 = models/old_cg_model.py:303-351): ``c`` holds the per-batch
+    constants (bonds, segment pointers, capacities); ``sync_free`` selects the capacity-buffer bond graph."""
+    lig = data['ligand']
+    ns, B = model.ns, data.num_graphs
+    n_lig = lig_node.shape[0]
+    # -- translation / rotation head (:368-395) -----------------------------------------------------------------
+    pos = lig.pos.float()
+    arange = torch.arange(n_lig, device=pos.device)
+    center = torch.zeros((B, 3), device=pos.device).index_add_(0, lig.batch, pos)
+    center = center / c['lig_cnt_f']
+    c_vec = pos - center[lig.batch]
+    c_ea = torch.cat([model.center_distance_expansion(c_vec.norm(dim=-1)), lig.node_sigma_emb], 1)
+    c_ea = model.center_edge_embedding(c_ea)
+    idx = arange if model.fixed_center_conv else lig.batch            # hazard C.6: graph id indexes lig_node
+    c_ea = torch.cat([c_ea, lig_node[idx, :ns]], -1)
+    glob = model.final_conv(lig_node, torch.stack([lig.batch, arange]), c_ea, None, out_nodes=B, edge_vec=c_vec,
+                            assume_sorted=True)
+    tr_pred = glob[:, :3] + (glob[:, 6:9] if not model.odd_parity else 0)
+    rot_pred = glob[:, 3:6] + (glob[:, 9:] if not model.odd_parity else 0)
+    data.graph_sigma_emb = model.timestep_emb_func(data.complex_t['tr'])
+    tr_norm = torch.linalg.vector_norm(tr_pred, dim=1).unsqueeze(1)
+    tr_pred = tr_pred / tr_norm * model.tr_final_layer(torch.cat([tr_norm, data.graph_sigma_emb], dim=1))
+    rot_norm = torch.linalg.vector_norm(rot_pred, dim=1).unsqueeze(1)
+    rot_pred = rot_pred / rot_norm * model.rot_final_layer(torch.cat([rot_norm, data.graph_sigma_emb], dim=1))
+    if model.scale_by_sigma:
+        tr_pred = tr_pred / tr_sigma.unsqueeze(1)
+        rot_pred = rot_pred * model._so3_score_norm(rot_sigma).unsqueeze(1)
+
+    if model.no_torsion or c['n_bonds'] == 0:
+        return tr_pred, rot_pred, torch.empty(0, device=model.device)
+
+    # -- torsion head (:406-423) --------------------------------------------------------------------------------
+    bonds = c['bonds']
+    n_bonds = c['n_bonds']
+    bond_pos = ((pos[bonds[0]] + pos[bonds[1]]) / 2).contiguous()
+    if sync_free:
+        # upper-bound buffer (32 atoms per bond, models/cg_model.py:630); slots beyond the live count point at an extra
+        # dummy bond row (index n_bonds) that is dropped after the convolution
+        pos_c = pos.contiguous()
+        cnt = ops.radius_count(pos_c, bond_pos, c['lig_ptr'], c['bond_batch32'], r=model.lig_max_radius, max_num_neighbors=32)
+        incl = torch.cumsum(cnt, 0, dtype=torch.int32)
+        bi32, ai32, t_vec, _, _ = ops.graph_fill(pos_c, bond_pos, c['lig_ptr'], c['bond_batch32'], (incl - cnt).contiguous(),
+                                                 c['cap_tor'], r=model.lig_max_radius, max_num_neighbors=32, fill_row=n_bonds)
+        bi, ai = bi32.long(), ai32.long()
+        bi_g = bi.clamp_max(n_bonds - 1)            # gathers of per-bond quantities for the dummy slots: any valid row
+        n_out = n_bonds + 1
+    else:
+        bi, ai, _ = ops.radius(pos, bond_pos, c['lig_ptr'], c['bond_batch'], r=model.lig_max_radius, max_num_neighbors=32)
+        bi, ai = bi.long(), ai.long()
+        t_vec = pos[ai] - bond_pos[bi]
+        bi_g, n_out = bi, n_bonds
+    t_ea = model.final_edge_embedding(model.lig_distance_expansion(t_vec.norm(dim=-1)))
+    bond_vec = pos[bonds[1]] - pos[bonds[0]]
+    bond_attr = lig_node[bonds[0]] + lig_node[bonds[1]]
+    t_sh = torch.einsum('ea,eb,abc->ec', _sh_full(t_vec, model.sh_lmax), _sh_l2(bond_vec)[bi_g], model._tor_tp)
+    t_ea = torch.cat([t_ea, lig_node[ai, :ns], bond_attr[bi_g, :ns]], -1)
+    tor_pred = model.tor_bond_conv(lig_node, torch.stack([bi, ai]), t_ea, t_sh, out_nodes=n_out, reduce='mean',
+                                   edge_weight=model.get_edge_weight(t_vec, model.lig_max_radius), assume_sorted=True)
+    tor_pred = model.tor_final_layer(tor_pred[:n_bonds]).squeeze(1)
+    edge_sigma = tor_sigma[c['bond_lig_batch']]
+    if model.scale_by_sigma:
+        tor_pred = tor_pred * torch.sqrt(model._torus_score_norm(edge_sigma))
+    return tr_pred, rot_pred, tor_pred
 
 
 class GaussianSmearing(nn.Module):

@@ -1,30 +1,67 @@
-"""Drop-in for the reference's confidence model ``models/old_cg_model.py:CGOldModel`` in confidence mode - the ranking
-model ``utils/sampling.py:208-227`` calls once per batch of final poses (SURVEY.md section 8, row f2).
+"""Drop-in for the reference's ``models/old_cg_model.py:CGOldModel``, the DiffDock v1.0 architecture, in both modes:
 
-Same constructor keywords, ``forward(data) -> confidence [B]`` (``[B, 2]`` with affinity_prediction) and ``state_dict``
-keys as the reference class for: confidence_mode=True, use_old_atom_encoder=True (the only encoder the reference class
-can be built with - its new AtomEncoder rejects the ``lm_embedding_type`` keyword, models/old_cg_model.py:63-66), no
-miscellaneous atoms, one noise schedule.  The convolutions are the same sm_90a kernels as the score model's: every
-OldTensorProductConvLayer call goes through the fully fused wgmma kernel (csrc/fused_conv.cu) when its shapes allow,
-neighbour lists come from ddb200_radius_*, spherical harmonics are evaluated in-kernel from the edge vectors.
+* confidence mode - the ranking model ``utils/sampling.py:208-227`` calls once per batch of final poses (SURVEY.md
+  section 8, row f2): ``forward(data) -> confidence [B]`` (``[B, 2]`` with affinity_prediction);
+* score mode - the v1.0 score model (``inference.py --old_score_model``): ``forward(data) -> (tr [B, 3], rot [B, 3],
+  tor [n_rotatable_bonds])``, the reference's 3-tuple.
+
+Same constructor keywords and ``state_dict`` keys as the reference class for: use_old_atom_encoder=True (the only encoder the
+reference class can be built with - its new AtomEncoder rejects the ``lm_embedding_type`` keyword,
+models/old_cg_model.py:63-66), no miscellaneous atoms, one noise schedule.  The convolutions are the same sm_90a kernels as
+the v1.1 score model's: every OldTensorProductConvLayer call goes through the fully fused wgmma kernel (csrc/fused_conv.cu)
+when its shapes allow, neighbour lists come from ddb200_radius_* / ddb200_graph_fill, spherical harmonics are evaluated
+in-kernel from the edge vectors.
+
+Score mode follows diffdock_b200.cg_model.CGModel: per-batch constants in ``_static``, a forward without any device->host
+read (``_forward_sync_free``, capturable in a CUDA graph by diffdock_b200.sampling) when every convolution has a fused-kernel
+shape, else ``_forward_host_sized``.  What the v1.0 wiring changes on that path (models/old_cg_model.py:203-351):
+
+1. sigma enters the receptor embeddings.  The node encoder is affine in the sigma embedding, so its sigma-free part
+   (including the 1280-wide language-model Linear) is computed once per batch and each step adds ``M . sigma_emb`` per
+   complex (``M`` [ns, S] folded from the encoder's weights); the contact-edge embedding runs in ddb200_edge_embed with
+   the sigma half of its first Linear applied per complex.  A batch of B poses of one receptor at one time embeds one
+   copy's contact graph and the copies read it through ``edge_perm``.
+2. Four convolutions per layer, each with its own radial MLP, mean and BatchNorm, residual=False: each is one fused launch
+   over the joint [ligand | residues] numbering into one of two accumulators (intra: lig<-lig and rec<-rec; inter:
+   lig<-rec and rec<-lig), and two chained ddb200_tpconv_finalize calls per node type give
+   ``pad(x) + BN_intra(mean_intra) + BN_inter(mean_inter)``.  The receptor is not updated in the last layer.
+3. The rec<-lig convolution reads ``[ea | node[lig] | node[rec]]`` while its target is the residue: the two node blocks of
+   its first Linear are swapped in the kernel plan (TensorProductConvLayer._fused_plan).
+4. rec<-lig uses Y(rec - lig) unnegated (:265): the reverse permutation of the cross list with ``vec_sign = +1``.
+5. Layer-0 rec<-rec messages of a one-receptor, one-time batch are computed for one copy and added to all copies.
 
 CUDA only, inference only.  No CPU fallback.
 """
 from __future__ import annotations
 
+import os
+
+import numpy as np
 import torch
 import torch.nn.functional as F
 from torch import nn
 
 from . import ops
+from .cg_model import _TABLES, CGModel, _flat, _i32
 from .irreps import irreps_str, sh_irreps
 from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_forward, confidence_head, cross_cutoff, cross_graph,
-                     edge_weight, ligand_graph)
+                     edge_weight, ligand_graph, score_heads)
 from .synthetic import LIG_FEATURE_DIMS as lig_feature_dims, REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims
 from .tensor_layers import OldTensorProductConvLayer
+from .tp_table import full_tensor_product
 
 
 class CGOldModel(nn.Module):
+    # The ligand and cross graphs, the score-norm look-ups and the per-batch constants of the sync-free path are the v1.1
+    # score model's (models/old_cg_model.py:361-391,439-461 = models/cg_model.py:467-497,539-562).
+    _static_sync_free = CGModel._static_sync_free
+    _ligand_edges_sync_free = CGModel._ligand_edges_sync_free
+    _cross_graph_sync_free = CGModel._cross_graph_sync_free
+    _cross_edge_embedding = CGModel._cross_edge_embedding
+    _edge_embed_in_kernel = CGModel._edge_embed_in_kernel
+    _so3_score_norm, _torus_score_norm = CGModel._so3_score_norm, CGModel._torus_score_norm
+    set_score_norm_tables = CGModel.set_score_norm_tables
+
     def __init__(self, t_to_sigma, device, timestep_emb_func, in_lig_edge_features=4, sigma_embed_dim=32, sh_lmax=2,
                  ns=16, nv=4, num_conv_layers=2, lig_max_radius=5, rec_max_radius=30, cross_max_distance=250,
                  center_max_distance=30, distance_embed_dim=32, cross_distance_embed_dim=32, no_torsion=False,
@@ -38,9 +75,6 @@ class CGOldModel(nn.Module):
         super().__init__()
         assert parallel == 1, "not implemented"
         assert (not no_aminoacid_identities) or (lm_embedding_type is None), "no language model emb without identities"
-        if not confidence_mode:
-            raise NotImplementedError("diffdock_b200.CGOldModel is built in confidence mode only (SURVEY.md row f2); "
-                                      "the score model is diffdock_b200.cg_model.CGModel")
         if not use_old_atom_encoder:
             raise NotImplementedError("models/old_cg_model.py can only be constructed with use_old_atom_encoder=True")
         if include_miscellaneous_atoms or separate_noise_schedule or asyncronous_noise_schedule or use_second_order_repr:
@@ -54,6 +88,8 @@ class CGOldModel(nn.Module):
         self.ns, self.nv, self.smooth_edges = ns, nv, smooth_edges
         self.confidence_mode, self.num_conv_layers = confidence_mode, num_conv_layers
         self.affinity_prediction, self.no_aminoacid_identities = affinity_prediction, no_aminoacid_identities
+        self.scale_by_sigma, self.no_torsion, self.odd_parity = scale_by_sigma, no_torsion, odd_parity
+        self.fixed_center_conv = fixed_center_conv
         kw = dict(lm_embedding_dim=lm_embedding_dim) if lm_embedding_type is not None else {}
         self.lig_node_embedding = OldAtomEncoder(ns, lig_feature_dims, sigma_embed_dim)
         self.lig_edge_embedding = _mlp(in_lig_edge_features + sigma_embed_dim + distance_embed_dim, ns, ns, dropout)
@@ -77,26 +113,221 @@ class CGOldModel(nn.Module):
             r2l.append(OldTensorProductConvLayer(**p))
         self.lig_conv_layers, self.rec_conv_layers = nn.ModuleList(lig), nn.ModuleList(rec)
         self.lig_to_rec_conv_layers, self.rec_to_lig_conv_layers = nn.ModuleList(l2r), nn.ModuleList(r2l)
-        bn = (lambda: nn.Identity()) if confidence_no_batchnorm else (lambda: nn.BatchNorm1d(ns))
-        self.confidence_predictor = nn.Sequential(
-            nn.Linear(2 * ns if num_conv_layers >= 3 else ns, ns), bn(), nn.ReLU(), nn.Dropout(confidence_dropout),
-            nn.Linear(ns, ns), bn(), nn.ReLU(), nn.Dropout(confidence_dropout),
-            nn.Linear(ns, 2 if affinity_prediction else 1))
+        if confidence_mode:
+            bn = (lambda: nn.Identity()) if confidence_no_batchnorm else (lambda: nn.BatchNorm1d(ns))
+            self.confidence_predictor = nn.Sequential(
+                nn.Linear(2 * ns if num_conv_layers >= 3 else ns, ns), bn(), nn.ReLU(), nn.Dropout(confidence_dropout),
+                nn.Linear(ns, ns), bn(), nn.ReLU(), nn.Dropout(confidence_dropout),
+                nn.Linear(ns, 2 if affinity_prediction else 1))
+            return
+        # score mode: translation / rotation and torsion heads (:156-201)
+        S, D = sigma_embed_dim, distance_embed_dim
+        self.center_distance_expansion = GaussianSmearing(0.0, center_max_distance, D)
+        self.center_edge_embedding = _mlp(D + S, ns, ns, dropout)
+        self.final_conv = OldTensorProductConvLayer(in_irreps=self.lig_conv_layers[-1].out_irreps, sh_irreps=self.sh_irreps,
+                                                    out_irreps='2x1o + 2x1e' if not odd_parity else '1x1o + 1x1e',
+                                                    n_edge_features=2 * ns, residual=False, dropout=dropout,
+                                                    batch_norm=batch_norm)
+        self.tr_final_layer = nn.Sequential(nn.Linear(1 + S, ns), nn.Dropout(dropout), nn.ReLU(), nn.Linear(ns, 1))
+        self.rot_final_layer = nn.Sequential(nn.Linear(1 + S, ns), nn.Dropout(dropout), nn.ReLU(), nn.Linear(ns, 1))
+        if not no_torsion:
+            self.final_edge_embedding = _mlp(D, ns, ns, dropout)
+            T, tor_sh = full_tensor_product(self.sh_irreps, '1x2e')       # o3.FullTensorProduct(sh, "2e"), :186
+            self.register_buffer('_tor_tp', torch.from_numpy(T).float(), persistent=False)
+            self.tor_bond_conv = OldTensorProductConvLayer(in_irreps=self.lig_conv_layers[-1].out_irreps,
+                                                           sh_irreps=irreps_str(tor_sh),
+                                                           out_irreps=f'{ns}x0o + {ns}x0e' if not odd_parity else f'{ns}x0o',
+                                                           n_edge_features=3 * ns, residual=False, dropout=dropout,
+                                                           batch_norm=batch_norm)
+            self.tor_final_layer = nn.Sequential(nn.Linear(2 * ns if not odd_parity else ns, ns, bias=False), nn.Tanh(),
+                                                 nn.Dropout(dropout), nn.Linear(ns, 1, bias=False))
+        z = np.load(_TABLES)        # score-norm tables (utils/so3.py:59, utils/torus.py:72-76), not in the state_dict
+        self.register_buffer('_so3_table', torch.from_numpy(z['so3_exp_score_norms']).float(), persistent=False)
+        self.register_buffer('_torus_table', torch.from_numpy(z['torus_score_norm']).float(), persistent=False)
+        self._sync_free = None
 
     def load_state_dict(self, state_dict, strict=True, **kw):
-        """Reference checkpoints carry e3nn's tensor-product buffers (``*.tp.*``): dropped, the kernels have their own tables."""
-        sd = {k: v for k, v in state_dict.items() if '.tp.' not in k}
+        """Reference checkpoints carry e3nn's tensor-product buffers (``*.tp.*``, and ``final_tp_tor.*`` in score mode):
+        dropped, the kernels have their own tables."""
+        sd = {k: v for k, v in state_dict.items() if '.tp.' not in k and not k.startswith('final_tp_tor.')}
         return super().load_state_dict(sd, strict=strict, **kw)
 
     def get_edge_weight(self, edge_vec, max_norm):                      # models/old_cg_model.py:353-359
         return edge_weight(edge_vec, max_norm, self.smooth_edges)
 
     @torch.no_grad()
-    def forward(self, data):                                            # models/old_cg_model.py:203-301
+    def forward(self, data):                                            # models/old_cg_model.py:203-351
         check_forward(self, data)
+        if self.confidence_mode:                                        # times are used as they are (:210)
+            return confidence_head(self, data, self._forward_host_sized(data, data.complex_t['tr']))
+        c = self._static(data)
+        tr_sigma, rot_sigma, tor_sigma = self.t_to_sigma(*[data.complex_t[k] for k in ('tr', 'rot', 'tor')])
+        sync_free = self.sync_free_capable() and c['rec_max'] <= 10000      # the cross graph's cap (:445) must not bind
+        lig_node = self._forward_sync_free(data, c, tr_sigma) if sync_free else self._forward_host_sized(data, tr_sigma)
+        return score_heads(self, data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_free)
+
+    def sync_free_capable(self):
+        """Score mode: the forward runs without any host synchronisation (and so inside a CUDA graph) when every
+        convolution of the stack has a shape the fully fused kernel supports."""
+        if self._sync_free is None:
+            ok = os.environ.get('DDB200_SYNC_FREE', '1') != '0'
+            for convs in (self.lig_conv_layers, self.rec_conv_layers, self.lig_to_rec_conv_layers, self.rec_to_lig_conv_layers):
+                ok = ok and all(layer.fused_capable(self.ns, self.ns) for layer in convs)
+            self._sync_free = bool(ok)
+        return self._sync_free
+
+    def sync_free_crop_capable(self):
+        """Per-step receptor cropping is not built into the sync-free v1.0 forward: ``crop_beyond`` runs the eager
+        ``sampling.crop_receptor`` path."""
+        return False
+
+    # ---------------------------------------------------------------------------------------------------------
+    def _static(self, data):
+        """Per-batch constants of the score model, cached on ``data`` (one host read per batch): the sigma-free part of the
+        receptor node embedding, the contact graph in CSR order by target, and those of CGModel._static_sync_free."""
+        rec, rr, lig, ll = data['receptor'], data['receptor', 'receptor'], data['ligand'], data['ligand', 'ligand']
+        if hasattr(rr, '_b200_v10'):
+            return rr._b200_v10
+        B, n_lig, ns = data.num_graphs, lig.batch.shape[0], self.ns
+        ei = rr.edge_index.long()
+        uniq = getattr(rec, '_unique', None)       # (nodes, edges, copies): the batch holds `copies` identical receptors
+        if uniq is not None and uniq[2] == B and uniq[0] * B == rec.pos.shape[0] and uniq[1] * B == ei.shape[1]:
+            copies, n1, e1 = B, uniq[0], uniq[1]
+        else:
+            copies, n1, e1 = 1, rec.pos.shape[0], ei.shape[1]
+        c = {'copies': copies}
+        # receptor node embedding with the sigma embedding set to zero (:401, :221), one copy, 1280-wide LM layer included
+        x1 = rec.x[:n1].float()
+        base = self.rec_node_embedding(torch.cat([x1, x1.new_zeros((n1, self.sigma_embed_dim))], 1))
+        c['rec_base'] = base.repeat(copies, 1) if copies > 1 else base
+        c['rec_sigma_map'] = self._rec_sigma_map(rec.x.shape[1])
+        c['rec_gid'] = rec.batch                # complex of each residue: the sigma terms are per complex, not per batch
+        # contact graph in CSR order by target (edge_index[0]); vector gathered - target (:406)
+        tgt, order = torch.sort(ei[0], stable=True)
+        src = ei[1][order]
+        pos = rec.pos.float()
+        vec = (pos[src] - pos[tgt]).contiguous()
+        ew = self.get_edge_weight(vec, self.rec_max_radius)
+        c['rr_tgt'], c['rr_src'], c['rr_vec'] = tgt, src, vec
+        c['rr_ew'] = _flat(ew)
+        c['rr_tgt_batch'] = rec.batch[tgt]
+        c['rr_joint'] = (_i32(tgt + n_lig), _i32(src + n_lig))
+        if copies > 1:      # copy 0 of the sorted contact graph (its targets sort first), local numbering
+            c['rr0'] = (_i32(tgt[:e1]), _i32(src[:e1]), vec[:e1].contiguous(),
+                        c['rr_ew'][:e1].contiguous() if c['rr_ew'] is not None else None)
+            c['rr0_row'] = torch.zeros(e1, dtype=torch.int32, device=vec.device)
+            c['rr_perm'] = _i32(torch.arange(ei.shape[1], device=vec.device) % e1)
+        c['rec_ptr'] = ops.segment_ptr(rec.batch, B)
+        c['lig_ptr'] = ops.segment_ptr(lig.batch, B)
+        bonds = ll.edge_index[:, lig.edge_mask].long()
+        c['bonds'], c['n_bonds'] = bonds, int(bonds.shape[1])
+        c['bond_batch'] = lig.batch[bonds[0]] if bonds.shape[1] else None
+        self._static_sync_free(data, c)
+        rr._b200_v10 = c
+        return c
+
+    def _rec_sigma_map(self, x_cols):
+        """``M`` [ns, S] with rec_node_embedding(cat[x, s]) = rec_node_embedding(cat[x, 0]) + M s for the encoder input
+        ``cat[x (x_cols columns), sigma embedding]``: the encoder reads its scalar columns and (with an LM embedding) the
+        last ``lm_embedding_dim`` columns of that input (models/layers.py:103-116); the sigma columns can fall in either."""
+        enc, S = self.rec_node_embedding, self.sigma_embed_dim
+        nc, nsf = enc.num_categorical_features, enc.num_scalar_features
+        cols = torch.arange(x_cols, x_cols + S)                              # where the sigma embedding sits
+        W = enc.linear.weight.detach()
+        m = W.new_zeros((W.shape[0], S))
+        j = cols - nc
+        ok = (j >= 0) & (j < nsf)
+        m[:, ok] = W[:, j[ok]]
+        if enc.lm_embedding_type is not None:
+            W_lm, lm = enc.lm_embedding_layer.weight.detach(), enc.lm_embedding_dim
+            m = W_lm[:, :W.shape[0]] @ m
+            j = cols - (x_cols + S - lm)
+            ok = j >= 0
+            m[:, ok] += W_lm[:, W.shape[0] + j[ok]]
+        return m.contiguous()
+
+    def _forward_sync_free(self, data, c, tr_sigma):
+        """Ligand node features after the interaction layers without a device->host read: capacity buffers with device
+        counts for the ligand and cross graphs (as CGModel._forward_sync_free), the receptor embeddings from the per-batch
+        constants plus the per-complex sigma terms, four fused convolutions per layer finalised per node type."""
+        lig, rec = data['ligand'], data['receptor']
+        ns, n_lig, B = self.ns, lig.batch.shape[0], data.num_graphs
+        shared = c['copies'] > 1 and getattr(data, '_uniform_t', False)     # one receptor at one diffusion time
+        sig = self.timestep_emb_func(data.complex_t['tr'])                    # [B, S], per complex
+
+        # -- receptor embeddings (:393-414) -------------------------------------------------------------------------------
+        rec_node = c['rec_base'] + (sig @ c['rec_sigma_map'].t())[c['rec_gid']]
+        if shared:      # one copy's contact edges; the other copies read them through edge_perm
+            t0, s0, vec0, ew0 = c['rr0']
+            ea0 = self._rec_edge_attr(sig[:1], vec0, c['rr0_row'])
+            g_rr = (*c['rr_joint'], ea0, vec0, ew0, dict(edge_perm=c['rr_perm']))
+        else:
+            g_rr = (*c['rr_joint'], self._rec_edge_attr(sig, c['rr_vec'], c['rr_gid32']), c['rr_vec'], c['rr_ew'], {})
+
+        # -- ligand graph (:361-391) and cross graph (:439-461) ----------------------------------------------------------
+        g_ll = self._ligand_edges_sync_free(data, c)
+        lig_node = self.lig_node_embedding(torch.cat([lig.x.float(), lig.node_sigma_emb], 1))
+        r, rpg = cross_cutoff(self, tr_sigma)
+        # rec <- lig reuses the lig <- rec attributes and harmonics Y(rec - lig) (:264-265): vec_sign = +1
+        g_lr, g_rl = self._cross_graph_sync_free(data, c, rec.pos.float().contiguous(), c['rec_ptr'], c['rec_batch32'],
+                                                 c['rec_max'], c['cap_cross'], r, rpg, n_lig, self.cross_edge_embedding,
+                                                 self.cross_distance_expansion, vec_sign=1.0)
+
+        # -- interaction layers (:247-294) --------------------------------------------------------------------------------
+        x = torch.cat([lig_node, rec_node], 0)
+        L = len(self.lig_conv_layers)
+        for l in range(L):
+            last = l == L - 1
+            n_out = n_lig if last else x.shape[0]
+            D = self.lig_conv_layers[l].out_size
+            intra = (torch.zeros((n_out, D), device=x.device), torch.zeros((n_out,), device=x.device))
+            inter = (torch.zeros((n_out, D), device=x.device), torch.zeros((n_out,), device=x.device))
+            self.lig_conv_layers[l].accumulate_group(x, g_ll, 0, n_out, ns, init=intra)
+            self.rec_to_lig_conv_layers[l].accumulate_group(x, g_lr, 0, n_out, ns, init=inter)
+            if not last:
+                if l == 0 and shared:
+                    self._shared_receptor_messages(x, c, n_lig, ea0, intra)
+                else:
+                    self.rec_conv_layers[l].accumulate_group(x, g_rr, 0, n_out, ns, init=intra)
+                self.lig_to_rec_conv_layers[l].accumulate_group(x, g_rl, 0, n_out, ns, init=inter, swap_gathered=True)
+            out = torch.empty((n_out, D), device=x.device)
+            rows = [(slice(0, n_lig), self.lig_conv_layers[l], self.rec_to_lig_conv_layers[l])]
+            if not last:
+                rows.append((slice(n_lig, n_out), self.rec_conv_layers[l], self.lig_to_rec_conv_layers[l]))
+            for sl, conv_a, conv_b in rows:      # pad(x) + BN_a(mean_a) + BN_b(mean_b)  (:281-290)
+                part = ops.tpconv_finalize(intra[0][sl], intra[1][sl], True, *self._bn(conv_a), residual=x[sl])
+                ops.tpconv_finalize(inter[0][sl], inter[1][sl], True, *self._bn(conv_b), residual=part, out=out[sl])
+            x = out
+        return x
+
+    def _rec_edge_attr(self, sig, vec, row):
+        """rec_edge_embedding(cat[sigma_emb of the edge's complex, rbf(|vec|)]) (:409-410, :222) with ``sig`` [rows, S] and
+        ``row`` the sigma row of each edge; a receptor without contact edges (e.g. cropped to a few residues) has none."""
+        if vec.shape[0] == 0:
+            return vec.new_zeros((0, self.ns))
+        return self._cross_edge_embedding(sig, vec, row, None, self.rec_edge_embedding, self.rec_distance_expansion)
+
+    @staticmethod
+    def _bn(layer):
+        return layer.batch_norm.fold() if layer.batch_norm is not None else (None, None)
+
+    def _shared_receptor_messages(self, x, c, n_lig, ea0, acc):
+        """Layer-0 rec <- rec messages of a batch of B poses of ONE receptor at ONE diffusion time (``data._uniform_t``):
+        the residue features and contact edges (attributes ``ea0`` of copy 0) entering the first layer are the same in
+        every copy, so the messages are computed for copy 0 and added to every copy's rows of ``acc``."""
+        t0, s0, vec0, ew0 = c['rr0']
+        B, n1 = c['copies'], (x.shape[0] - n_lig) // c['copies']
+        sum0, cnt0 = self.rec_conv_layers[0].accumulate_group(x[n_lig:n_lig + n1], (t0, s0, ea0, vec0, ew0, {}), 0, n1,
+                                                              self.ns)
+        acc[0][n_lig:].view(B, n1, -1).add_(sum0.unsqueeze(0))
+        acc[1][n_lig:].view(B, n1).add_(cnt0.unsqueeze(0))
+
+    def _forward_host_sized(self, data, tr_sigma):
+        """Ligand node features after the interaction layers, with exactly-sized neighbour lists (one host read of each
+        edge count) and every convolution through OldTensorProductConvLayer.forward: the confidence model, and the score
+        model when a convolution shape is outside the fused kernel's templates."""
         lig, rec = data['ligand'], data['receptor']
         B, ns = data.num_graphs, self.ns
-        tr_sigma = data.complex_t['tr']                                 # confidence mode: times are used as they are
         rp = rec.pos.float()
 
         # ligand graph (:361-391): bonds + radius graph; row 0 = convolution target, row 1 = gathered node
@@ -137,4 +368,4 @@ class CGOldModel(nn.Module):
             lig_node = F.pad(lig_node, (0, lig_intra.shape[-1] - lig_node.shape[-1])) + lig_intra + lig_inter
             if l != L - 1:
                 rec_node = F.pad(rec_node, (0, rec_intra.shape[-1] - rec_node.shape[-1])) + rec_intra + rec_inter
-        return confidence_head(self, data, lig_node)
+        return lig_node

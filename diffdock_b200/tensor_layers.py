@@ -180,16 +180,22 @@ class TensorProductConvLayer(nn.Module):
             self._fcache[id(fc)] = hit
         return hit[1:]
 
-    def _fused_plan(self, fc, table, k_in):
-        """Plan of the fully fused kernel for this radial MLP, or None when the shapes are outside its templates."""
+    def _fused_plan(self, fc, table, k_in, swap_ns=0):
+        """Plan of the fully fused kernel for this radial MLP, or None when the shapes are outside its templates.
+        ``swap_ns`` > 0: the MLP was trained on ``[ea | node[src] | node[tgt]]`` (ns columns each) while the kernel assembles
+        ``[ea | node[tgt] | node[src]]``, so the two node blocks of the first Linear's columns trade places in the plan."""
         if not (fused.ENABLED and self._fusable(fc, k_in) and fused.supported(table, fc[0].out_features, k_in)):
             return None
         l1, l2 = fc[0], fc[-1]
         key = (l1.weight._version, l1.bias._version, l2.weight._version, l2.bias._version, l2.weight.device)
-        hit = self._pcache.get(id(fc))
+        hit = self._pcache.get((id(fc), swap_ns))
         if hit is None or hit[0] != key:
-            hit = (key, fused.FusedPlan(table, l1.weight, l1.bias, l2.weight, l2.bias))
-            self._pcache[id(fc)] = hit
+            w1 = l1.weight
+            if swap_ns:
+                ne = k_in - 2 * swap_ns
+                w1 = torch.cat([w1[:, :ne], w1[:, ne + swap_ns:], w1[:, ne:ne + swap_ns]], 1)
+            hit = (key, fused.FusedPlan(table, w1, l1.bias, l2.weight, l2.bias))
+            self._pcache[(id(fc), swap_ns)] = hit
         return hit[1]
 
     @staticmethod
@@ -309,17 +315,20 @@ class TensorProductConvLayer(nn.Module):
         return self._run(x, prepared, fcs, True, 1.0, n_out, reduce, gather_scalars, scale, shift, init=init)
 
     @torch.no_grad()
-    def accumulate_group(self, node_attr, group, group_index, n_out, gather_scalars=0):
+    def accumulate_group(self, node_attr, group, group_index, n_out, gather_scalars=0, init=None, swap_gathered=False):
         """Raw accumulators ``(sum [n_out, D_out], cnt [n_out])`` of ONE edge group (radial MLP ``group_index`` of this layer)
         without the mean / BatchNorm / residual epilogue - for messages that are shared by several target blocks (the
         receptor<-receptor messages of the first interaction layer are identical for all poses of a complex) and are added to
-        the layer's accumulators through ``forward_groups(..., init=...)``."""
+        the layer's accumulators through ``forward_groups(..., init=...)``, or that are finalised by the caller.  ``init``:
+        accumulators to add to (returned) instead of fresh zeros.  ``swap_gathered``: the radial MLP reads the gathered node's
+        scalars before the target's (``[ea | node[src] | node[tgt]]``, models/old_cg_model.py:264-265); fused kernel only."""
         x = node_attr.float()
         if x.stride(1) != 1:
             x = x.contiguous()
         fcs = [self.fc] if self.edge_groups == 1 else list(self.fc)
         fc = fcs[0] if self.edge_groups == 1 else fcs[group_index]
-        return self._run(x, [group], [fc], True, 1.0, int(n_out), 'sum', gather_scalars, None, None, finalize=False)
+        return self._run(x, [group], [fc], True, 1.0, int(n_out), 'sum', gather_scalars, None, None, init=init,
+                         finalize=False, swap_gathered=swap_gathered)
 
     def fused_capable(self, k_edge, gather_scalars):
         """True if every radial MLP of this layer runs on the fully fused kernel for ``k_edge`` per-edge attribute columns
@@ -332,7 +341,7 @@ class TensorProductConvLayer(nn.Module):
         return all(fused.ENABLED and self._fusable(fc, k_in) and fused.supported(table, fc[0].out_features, k_in) for fc in fcs)
 
     def _run(self, x, prepared, fcs, from_vec, ew_scalar, n_out, reduce, gather_scalars, scale, shift, residual=None,
-             init=None, finalize=True):
+             init=None, finalize=True, swap_gathered=False):
         handle = self.tp.handle(from_vec)
         table = handle.table
         if init is not None:
@@ -349,8 +358,11 @@ class TensorProductConvLayer(nn.Module):
             extras = item[5] if len(item) > 5 else None
             n_e = tgt32.shape[0]
             k_in = ea.shape[1] + 2 * gather_scalars
-            plan = self._fused_plan(fc, table, k_in) \
+            plan = self._fused_plan(fc, table, k_in, gather_scalars if swap_gathered else 0) \
                 if (from_vec and ew_scalar == 1.0 and (n_e >= 64 or extras is not None)) else None
+            if swap_gathered and plan is None:
+                raise RuntimeError("swapped node scalars (swap_gathered) need a fused-kernel layer shape "
+                                   "(TensorProductConvLayer.fused_capable)")
             if plan is not None:      # radial MLP + tensor product + scatter in one kernel, no per-edge weights in HBM
                 fused.fused_conv(plan, ea.float(), x, gather_scalars, tgt32, src32, x, geo.float(), sum_buf, cnt_buf,
                                  edge_weight=ew.float().contiguous() if ew is not None else None, **(extras or {}))
