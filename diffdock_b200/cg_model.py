@@ -248,18 +248,14 @@ class CGModel(nn.Module):
         c['cap_cross'] = int((host[0].long() * host[1].long()).sum())      # every ligand atom x every residue of its complex
         c['lig_batch32'], c['rec_batch32'] = _i32(lig.batch), _i32(rec.batch)
         c['rr_gid32'] = _i32(c['rr_tgt_batch'])
-        # bond edges grouped by their convolution target (edge_index[0]), original order kept inside a group
+        # bond edges sorted by their convolution target (edge_index[0]), original order kept inside a target
         ei = ll.edge_index.long()
         order = torch.sort(ei[0], stable=True).indices
-        c['pre_col'] = _i32(ei[1][order])
-        cnt = torch.bincount(ei[0], minlength=n_lig)[:n_lig] if ei.shape[1] else torch.zeros(n_lig, dtype=torch.long, device=dev)
-        ptr = torch.zeros(n_lig + 1, dtype=torch.int32, device=dev)
-        ptr[1:] = torch.cumsum(cnt, 0)
-        c['pre_ptr'], c['pre_cnt'] = ptr, _i32(cnt)
+        c['pre_tgt'], c['pre_col'] = _i32(ei[0][order]), _i32(ei[1][order])
         attr = ll.edge_attr.float()[order] if ei.shape[1] else torch.zeros((0, self.in_lig_edge_features), device=dev)
         c['pre_attr'] = torch.cat([attr, torch.zeros((1, attr.shape[1]), device=dev)], 0)     # row -1: "not a bond"
-        # radius_graph(max_num_neighbors=32) = radius with cap 33 minus the self hit: an atom whose own index is not among its
-        # first 33 hits keeps 33 neighbours
+        # radius_graph(max_num_neighbors=32) = radius with cap 33 minus the self hit: a centre atom whose own index is not
+        # among its first 33 hits keeps 33 neighbours
         c['cap_ll'] = int(ei.shape[1]) + 33 * n_lig
         c['bond_lig_batch'] = lig.batch[c['bonds'][0]] if c['n_bonds'] else None
         c['cap_tor'] = 32 * c['n_bonds']
@@ -395,20 +391,36 @@ class CGModel(nn.Module):
 
     def _ligand_edges_sync_free(self, data, c):
         """The edge group of the ligand graph (bonds + radius graph, CSR by target) in a capacity buffer; sets
-        ``node_sigma_emb`` on the ligand."""
+        ``node_sigma_emb`` on the ligand.
+
+        radius_graph caps the neighbours of each CENTRE atom at 32, and its edges point from the centre to the neighbour,
+        which is the convolution's target (edge_index = [neighbour, centre], models/cg_model.py:478-483).  Where the cap
+        binds, an atom can be the target of more than 32 edges, so the search runs per centre and the pairs are then
+        sorted by target: the bonds of each target first (in their original order), then its radius edges by centre, the
+        order of the reference's concatenation sorted stably by target."""
         lig = data['ligand']
         pos = lig.pos.float().contiguous()
+        n_lig = pos.shape[0]
         lig.node_sigma_emb = self.timestep_emb_func(lig.node_t['tr'])
         cnt = ops.radius_count(pos, pos, c['lig_ptr'], c['lig_batch32'], r=self.lig_max_radius, max_num_neighbors=33,
-                               exclude_self=True) + c['pre_cnt']
+                               exclude_self=True)
         incl = torch.cumsum(cnt, 0, dtype=torch.int32)
-        tgt, src, vec, eid, _ = ops.graph_fill(
-            pos, pos, c['lig_ptr'], c['lig_batch32'], (incl - cnt).contiguous(), c['cap_ll'], r=self.lig_max_radius,
-            max_num_neighbors=33, exclude_self=True, pre_ptr=c['pre_ptr'], pre_col=c['pre_col'], want_eid=True, fill_row=0)
-        attr = torch.cat([c['pre_attr'][eid.long()], lig.node_sigma_emb[tgt.long()],
+        n_b = c['pre_col'].shape[0]
+        centre, nbr, _, _, _ = ops.graph_fill(
+            pos, pos, c['lig_ptr'], c['lig_batch32'], (incl - cnt).contiguous(), c['cap_ll'] - n_b, r=self.lig_max_radius,
+            max_num_neighbors=33, exclude_self=True, want_vec=False, fill_row=0)
+        # rows past the live count get the key n_lig, so that they sort last
+        live = torch.arange(centre.shape[0], dtype=torch.int32, device=pos.device) < incl[-1:]
+        key = torch.cat([c['pre_tgt'], torch.where(live, nbr, n_lig)])
+        tgt, perm, _ = ops.csr_sort_by_target(key.contiguous(), n_lig + 1)
+        src = torch.cat([c['pre_col'], centre])[perm].contiguous()
+        eid = torch.cat([torch.arange(n_b, device=pos.device), torch.full_like(centre, -1, dtype=torch.long)])[perm]
+        tgt = torch.where(tgt < n_lig, tgt, 0).contiguous()              # padded rows: any valid node
+        vec = (pos[src.long()] - pos[tgt.long()]).contiguous()
+        attr = torch.cat([c['pre_attr'][eid], lig.node_sigma_emb[tgt.long()],
                           self.lig_distance_expansion(vec.norm(dim=-1))], 1)
         return (tgt, src, self.lig_edge_embedding(attr), vec, _flat(self.get_edge_weight(vec, self.lig_max_radius)),
-                dict(n_edges_dev=incl[-1:]))
+                dict(n_edges_dev=incl[-1:] + n_b))
 
     def _cross_graph_sync_free(self, data, c, xpos, x_ptr, x_batch32, x_max, cap, r, rpg, col_off, mlp, gs, vec_sign):
         """Ligand <- x edges (x: residues or receptor atoms at ``xpos``, numbered from ``col_off`` in the joint graph) in a

@@ -126,10 +126,14 @@ struct FusedParams {
 // channel is fixed up to a shift by 2 q, so every index into the partial sums is known at compile time), and NCOPY =
 // 8 / gcd(MULOUT, 8) threads of a quad hold partial sums of the same channel.
 template <int MULOUT> struct Slots {
-  static_assert(MULOUT % 2 == 0, "a column pair (b = 0, 1) lies in one row u");
+  static_assert(MULOUT % 2 == 0 && MULOUT >= 4, "a column pair (b = 0, 1) lies in one row u; w() wraps at most once");
   static constexpr int G = MULOUT % 8 == 0 ? 8 : (MULOUT % 4 == 0 ? 4 : 2);
   static constexpr int P = MULOUT / G, N = 2 * P, NCOPY = 8 / G;
-  static __device__ __forceinline__ int w(int slot, int q) { return (8 * (slot >> 1) + 2 * q + (slot & 1)) % MULOUT; }
+  // (8 (slot >> 1) + (slot & 1) + 2 q) mod MULOUT as a compile-time channel plus a shift: 2 q <= 6 wraps at most once
+  static __device__ __forceinline__ int w(int slot, int q) {
+    const int c = (8 * (slot >> 1) + (slot & 1)) % MULOUT;
+    return c + 2 * q - (2 * q >= MULOUT - c ? MULOUT : 0);
+  }
 };
 constexpr int NACC_MAX = 60;                     // partial sums per thread: slots x d_out x 2 edges, at most 10 x 3 x 2
 constexpr int ZLD = 68;                          // z buffer row of one edge: [16 rows u][4]; 8 edges' 16-byte reads hit 8 bank groups
@@ -147,7 +151,9 @@ __device__ __forceinline__ void contract(const Acc& d, const float* __restrict__
 #pragma unroll
   for (int j = 0; j < NCOL / 8; ++j) {
     if ((j >> 2) < nch) {
-      const int u = (MULOUT % 8 == 0) ? j / (MULOUT / 8) : (8 * j + 2 * q) / MULOUT;
+      // u = (8 j + 2 q) / MULOUT: 8 j splits into a compile-time row and remainder, and 2 q < 8 adds at most one row
+      const int JR = (8 * j) % MULOUT;
+      const int u = (8 * j) / MULOUT + ((MULOUT % 8 != 0 && 2 * q >= MULOUT - JR) ? 1 : 0);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float zk[3];
@@ -636,7 +642,9 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
         case 0: build_z<1, 4>(xn, d_in, M, zrow, ub); break;
         case 1: build_z<3, 16>(xn, d_in, M, zrow, ub); break;
         case 2: build_z<1, 8>(xn, d_in, M, zrow, ub); break;
-        default: build_z<3, 16>(xn, d_in, M, zrow, ub); break;
+        case 3: build_z<3, 16>(xn, d_in, M, zrow, ub); break;
+        case 4: case 5: build_z<1, 16>(xn, d_in, M, zrow, ub); break;
+        default: __trap();     // unreachable: FusedPlan writes kinds 0-5 only (fused.py:CONSUMER_KINDS)
       }
       __syncwarp();
       if (ti + 1 < p.n_tiles) prefetch_tile(xrow, tt + 8, ub, p.x_vec2, xn);
@@ -647,14 +655,20 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
         case 0: contract<48, 1, 4>(d, zcon, nch, q, acc); break;
         case 1: contract<10, 3, 16>(d, zcon, nch, q, acc); break;
         case 2: contract<16, 1, 8>(d, zcon, nch, q, acc); break;
-        default: contract<4, 3, 16>(d, zcon, nch, q, acc); break;
+        case 3: contract<4, 3, 16>(d, zcon, nch, q, acc); break;
+        case 4: contract<10, 1, 16>(d, zcon, nch, q, acc); break;
+        case 5: contract<4, 1, 16>(d, zcon, nch, q, acc); break;
+        default: __trap();
       }
       if (flags & 2) {
         switch (kind) {
           case 0: flush<48, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
           case 1: flush<10, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
           case 2: flush<16, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-          default: flush<4, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+          case 3: flush<4, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+          case 4: flush<10, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+          case 5: flush<4, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+          default: __trap();
         }
       }
       if (dwait) dwait[1] += (unsigned long long)(clock64() - c0);

@@ -9,6 +9,9 @@ whole rows ``u`` of one path block ``[mul_in, mul_out]``:
 
     (mul_out, 2l_out+1) = (48, 1): 4 rows x 48 columns = 192        (10, 3): 16 rows x 10 columns = 160
     (16, 1): 8 x 16 = 128                                            (4, 3): 16 x 4 = 64
+    (10, 1): 16 x 10 = 160                                           (4, 1): 16 x 4 = 64
+
+(the two ``(nv, 1)`` kinds are the ``nv x0o`` blocks that ``reduce_pseudoscalars`` gives layers 2 and up)
 
 so that a consumer thread (one edge = one accumulator row) knows at compile time which register of its accumulator every
 accumulator column feeds.  This module builds, from a ``TpTable`` and the radial MLP's second Linear:
@@ -34,7 +37,7 @@ from .radial import BK, BN
 from .tp_table import TpTable
 
 # (mul_out, d_out) -> (consumer kind id, rows per tile)
-CONSUMER_KINDS = {(48, 1): (0, 4), (10, 3): (1, 16), (16, 1): (2, 8), (4, 3): (3, 16)}
+CONSUMER_KINDS = {(48, 1): (0, 4), (10, 3): (1, 16), (16, 1): (2, 8), (4, 3): (3, 16), (10, 1): (4, 16), (4, 1): (5, 16)}
 MAX_K = 144          # widest radial-MLP input / hidden layer (16-column sections: 2 * 144 + 16 = 304 -> 5 k-blocks of 64)
 MAX_TILES = 128      # tile table capacity of the kernel (csrc/fused_conv.cu)
 MTAB = 48            # floats per path in the dense Clebsch-Gordan table: [3][3][5] padded
