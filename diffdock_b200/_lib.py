@@ -35,6 +35,7 @@ SIGNATURES = {
     'ddb200_radial_mlp': (_int, [_vp, _i64, _int, _vp, _i64, _int, _vp, _vp, _vp, _vp, _int, _vp, _vp, _int, _i64, _vp,
                                  _i64, _vp]),
     'ddb200_fused_conv': (_int, [_vp, _vp]),          # (const ddb200_fused_args*, stream)
+    'ddb200_fused_conv_so': (_int, [_vp, _vp]),       # (const ddb200_fused_args*, stream), second-order plans
     'ddb200_fused_debug_read': (_int, [_vp]),
     'ddb200_contact_count': (_int, [_vp, _i32, C.c_float, _i32, _i32, _vp, _vp]),
     'ddb200_contact_fill': (_int, [_vp, _i32, C.c_float, _i32, _i32, _vp, _vp, _vp, _vp]),

@@ -51,6 +51,10 @@ constexpr int OPS_PER_KB = 8;                    // MMAs that read one staged k-
 constexpr int THREADS = 256;                     // two warpgroups, each with its own 64 edges
 constexpr int MAX_TILES = 128, MAX_PATHS = 16, MTAB = 48;     // per path: dense [3][3][5] table, padded to 48 floats
 constexpr int BAR_WG = 1;                        // named barrier BAR_WG + g: the 128 threads of warpgroup g
+// Second-order instantiation (SO, node irreps with l = 2 blocks: use_second_order_repr): 5-component inputs and outputs, up
+// to 32 paths whose dense [5][5][5] tables (padded to 128 floats, 16 KB) are read through L1 instead of being staged, and
+// 3 B stages, so that the larger z buffer fits beside the two A images under the 227 KB opt-in.
+constexpr int SO_STAGES = 3, SO_MAX_PATHS = 32, SO_MTAB = 128;
 
 // fire-and-forget global reduction (atomicAdd here may be compiled to an atomic that returns its old value)
 __device__ __forceinline__ void red_add(float* addr, float v) {
@@ -138,16 +142,23 @@ template <int MULOUT> struct Slots {
 constexpr int NACC_MAX = 60;                     // partial sums per thread: slots x d_out x 2 edges, at most 10 x 3 x 2
 constexpr int ZLD = 68;                          // z buffer row of one edge: [16 rows u][4]; 8 edges' 16-byte reads hit 8 bank groups
 constexpr int WG_BUF = 64 * ZLD;                 // floats per warpgroup: z [64][ZLD], or the scatter staging [copies][64][nacc + 1]
+// SO: components 3, 4 of a 5-component z row lie in a second plane [64][ZLDB] behind the first ([16 rows u][2]; 8 edges'
+// 8-byte reads hit 16 distinct banks).  The scatter staging still fits in the first plane.
+constexpr int ZLDB = 34;
+constexpr int WG_BUF_SO = 64 * (ZLD + ZLDB);
 
 using Acc = float[MAX_N / 2];
 
-// acc[(slot d_out + k) 2 + h] += d[edge h, columns of the slot] * z[edge h][u][k] over the tile's first `nch` 32-column
-// chunks; z = the row of this thread's first edge in the z buffer (the second edge lies 8 rows further)
-template <int MULOUT, int DOUT, int ROWS>
-__device__ __forceinline__ void contract(const Acc& d, const float* __restrict__ z, int nch, int q, float* __restrict__ acc) {
+// acc[(slot d_out + k) 2 + h] += d[edge h, columns of the slot] * z[edge h][u][K0 + k] over the tile's first `nch` 32-column
+// chunks; z = the row of this thread's first edge in the z buffer (the second edge lies 8 rows further), zb its row in the
+// second plane (SO only: K0 + DOUT > 3)
+template <int MULOUT, int DOUT, int ROWS, int K0 = 0>
+__device__ __forceinline__ void contract(const Acc& d, const float* __restrict__ z, int nch, int q, float* __restrict__ acc,
+                                         const float* __restrict__ zb = nullptr) {
   using S = Slots<MULOUT>;
   constexpr int NCOL = MULOUT * ROWS;
   static_assert(NCOL % 32 == 0 && NCOL <= MAX_N && S::N * DOUT * 2 <= NACC_MAX, "tile width");
+  static_assert((K0 == 0 && (DOUT <= 3 || DOUT == 5)) || (K0 == 3 && DOUT == 2), "a z row is read as (0..2 | 3..4)");
 #pragma unroll
   for (int j = 0; j < NCOL / 8; ++j) {
     if ((j >> 2) < nch) {
@@ -156,12 +167,19 @@ __device__ __forceinline__ void contract(const Acc& d, const float* __restrict__
       const int u = (8 * j) / MULOUT + ((MULOUT % 8 != 0 && 2 * q >= MULOUT - JR) ? 1 : 0);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        float zk[3];
-        if (DOUT == 1) {
+        float zk[DOUT];
+        if constexpr (K0 == 3) {
+          const float2 v = *reinterpret_cast<const float2*>(zb + h * 8 * ZLDB + u * 2);
+          zk[0] = v.x; zk[1] = v.y;
+        } else if constexpr (DOUT == 1) {
           zk[0] = z[h * 8 * ZLD + u * 4];
         } else {
           const float4 v = *reinterpret_cast<const float4*>(z + h * 8 * ZLD + u * 4);
           zk[0] = v.x; zk[1] = v.y; zk[2] = v.z;
+          if constexpr (DOUT == 5) {
+            const float2 w = *reinterpret_cast<const float2*>(zb + h * 8 * ZLDB + u * 2);
+            zk[3] = w.x; zk[4] = w.y;
+          }
         }
 #pragma unroll
         for (int b = 0; b < 2; ++b) {
@@ -194,6 +212,31 @@ __device__ __forceinline__ void build_z(const float* __restrict__ xn, int d_in, 
   }
 }
 
+// SO: as build_z for d_in in {1, 3, 5} and DOUT in {1, 3, 5}, M = [5][5] (row-major, zero where i >= d_in or k >= d_out);
+// xs = the node values of rows u0 .. u0 + nrows - 1, read here rather than prefetched: the prefetch would hold 40 values
+// through the MMAs, while here they live beside the free accumulator registers only
+template <int DOUT, int ROWS>
+__device__ __forceinline__ void build_z_so(const float* __restrict__ xs, int nrows, int d_in, const float* __restrict__ M,
+                                           float* __restrict__ zrow, float* __restrict__ zrowb, int u0) {
+  constexpr int NU = ROWS < 8 ? ROWS : 8;
+  if (u0 >= ROWS) return;
+  float xv[NU][5];
+#pragma unroll
+  for (int r = 0; r < NU; ++r)
+#pragma unroll
+    for (int i = 0; i < 5; ++i) xv[r][i] = (r < nrows && i < d_in) ? __ldg(xs + r * d_in + i) : 0.f;
+#pragma unroll
+  for (int r = 0; r < NU; ++r) {
+    float z[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int k = 0; k < DOUT; ++k)
+#pragma unroll
+      for (int i = 0; i < 5; ++i) z[k] = fmaf(xv[r][i], M[5 * i + k], z[k]);
+    *reinterpret_cast<float4*>(zrow + (u0 + r) * 4) = make_float4(z[0], z[1], z[2], 0.f);
+    if (DOUT == 5) *reinterpret_cast<float2*>(zrowb + (u0 + r) * 2) = make_float2(z[3], z[4]);
+  }
+}
+
 constexpr int XN = 24;     // node values one thread gathers per tile: 8 rows x at most 3 components
 __device__ __forceinline__ void prefetch_x(const float* __restrict__ src, int cnt, int vec2, float* __restrict__ xn) {
   if (vec2) {          // 8-byte loads: every tile offset and count of the plan is even
@@ -217,8 +260,9 @@ __device__ __forceinline__ void prefetch_tile(const float* xrow, const int* ti, 
 // End of an output irrep: scatter-add of the warpgroup's 64 edges.  Every thread stages its partial sums in shared memory
 // (over the z buffer, at most two copies: with four, the pairs q, q ^ 1 are first added by a shuffle); warp w4 then takes edges 32 (w4 & 1) .. + 31 and output value i = 32 (w4 >> 1) + lane,
 // adds the copies, sums runs of equal targets (CSR order makes them contiguous; unsorted input just yields runs of length
-// one) and issues ONE fully coalesced RED.ADD per run for output value i.
-template <int MULOUT, int DOUT>
+// one) and issues ONE fully coalesced RED.ADD per run for output value i.  A slice (SO: components K0 .. K0 + DOUT - 1 of a
+// DFULL-component block) lands at w DFULL + K0 + k of the block.
+template <int MULOUT, int DOUT, int DFULL = DOUT, int K0 = 0>
 __device__ __forceinline__ void flush(const FusedParams& p, float* __restrict__ acc, float* buf, int r0, int q, int w4,
                                       int lane, int dst_s, uint32_t head_mask, int out_off, int bar) {
   using S = Slots<MULOUT>;
@@ -269,7 +313,12 @@ __device__ __forceinline__ void flush(const FusedParams& p, float* __restrict__ 
       for (int c = 0; c < NCOPY; ++c) s += col[(c * 64 + le) * LD];
       if (le == 31 || ((head_mask >> (le + 1)) & 1)) {          // warp-uniform: last edge of a run
         const int dst = __shfl_sync(0xffffffffu, dst_s, le);
-        if (dst >= 0 && act) red_add(p.sum + (long long)dst * p.d_out + out_off + i, s);
+        if constexpr (DFULL == DOUT) {
+          if (dst >= 0 && act) red_add(p.sum + (long long)dst * p.d_out + out_off + i, s);
+        } else {
+          const int w = i / DOUT;
+          if (dst >= 0 && act) red_add(p.sum + (long long)dst * p.d_out + out_off + w * DFULL + K0 + (i - w * DOUT), s);
+        }
         s = 0.f;
       }
     }
@@ -303,9 +352,9 @@ __device__ __forceinline__ void build_ops(uint32_t* ops, int S, uint32_t a_lo0) 
   }
 }
 
-// B stream of a CTA: per edge tile the W1' k-blocks, then every N tile's W2' k-blocks; item i goes to stage i % STAGES and
+// B stream of a CTA: per edge tile the W1' k-blocks, then every N tile's W2' k-blocks; item i goes to stage i % NST and
 // is read by both warpgroups
-struct Stream {
+template <int NST> struct Stream {
   unsigned char* sB; uint64_t* full; uint32_t* rel; const int* tiles;
   int n1, per_unit; uint32_t len;
   __device__ __forceinline__ void issue(const FusedParams& p, uint32_t i) const {
@@ -320,16 +369,16 @@ struct Stream {
       src = reinterpret_cast<const unsigned char*>(p.w2img) + (size_t)(j - p.n_kb1) * B_IMAGE_BYTES;
       bytes = (uint32_t)tiles[((j - p.n_kb1) / p.n_kb) * 8 + 1] * 128u;
     }
-    const uint32_t s = i % STAGES;
+    const uint32_t s = i % NST;
     bulk_load(sB + (size_t)s * STAGE_BYTES, src, bytes, &full[s]);
   }
   // item i has been read by every MMA of this warpgroup (its group is complete in every warp): the second warpgroup to
-  // release it refills its stage with item i + STAGES (rel[s] counts two releases per use of stage s)
+  // release it refills its stage with item i + NST (rel[s] counts two releases per use of stage s)
   __device__ __forceinline__ void release(const FusedParams& p, uint32_t i, int bar, int t) const {
     named_bar(bar, 128);
     if (t == 0) {
       __threadfence_block();
-      if (atomicAdd(rel + i % STAGES, 1u) & 1u) issue(p, i + STAGES);
+      if (atomicAdd(rel + i % NST, 1u) & 1u) issue(p, i + NST);
     }
   }
 };
@@ -354,14 +403,14 @@ __device__ __forceinline__ void mma_chain(Acc& d, const uint32_t* oa, const uint
   wgmma_commit();
 }
 
-// k-block kb of the schedule `ops` from stage mc % STAGES into d; dwait (debug, one thread per warpgroup) collects the
+// k-block kb of the schedule `ops` from stage mc % NST into d; dwait (debug, one thread per warpgroup) collects the
 // clocks spent waiting for the stage to land
-template <bool FIRST>
-__device__ __forceinline__ void mma_kblock(Acc& d, const Stream& st, const uint32_t* ops, int kb, uint32_t mc,
+template <bool FIRST, int NST>
+__device__ __forceinline__ void mma_kblock(Acc& d, const Stream<NST>& st, const uint32_t* ops, int kb, uint32_t mc,
                                            unsigned long long* dwait) {
-  const uint32_t s = mc % STAGES;
+  const uint32_t s = mc % NST;
   const long long c0 = dwait ? clock64() : 0;
-  mbar_wait(&st.full[s], (mc / STAGES) & 1);
+  mbar_wait(&st.full[s], (mc / NST) & 1);
   if (dwait) *dwait += (unsigned long long)(clock64() - c0);
   const uint32_t* oa = ops + kb * 2 * OPS_PER_KB;
   const uint32_t* ob = oa + OPS_PER_KB;
@@ -381,7 +430,8 @@ __device__ __forceinline__ void mma_kblock(Acc& d, const Stream& st, const uint3
 
 // one product, k-blocks 0 .. nkb - 1, into d.  Once a k-block is committed the previous one is waited for and released;
 // on return every group is complete, every stage the product read released and d readable.
-__device__ __forceinline__ void mma_product(Acc& d, const FusedParams& p, const Stream& st, const uint32_t* ops, int nkb, uint32_t& mc, int bar, int t, unsigned long long* dwait) {
+template <int NST>
+__device__ __forceinline__ void mma_product(Acc& d, const FusedParams& p, const Stream<NST>& st, const uint32_t* ops, int nkb, uint32_t& mc, int bar, int t, unsigned long long* dwait) {
   mma_kblock<true>(d, st, ops, 0, mc++, dwait);
   for (int kb = 1; kb < nkb; ++kb, ++mc) {
     mma_kblock<false>(d, st, ops, kb, mc, dwait);
@@ -504,32 +554,49 @@ __device__ __forceinline__ void build_a0(const FusedParams& p, unsigned char* sA
   fence_proxy_async();
 }
 
-__global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParams p) {
+// Shared-memory budget of an instantiation (the launcher checks it against the 227 KB opt-in): the two A images, the B
+// stages, the z / staging buffers, Y, the staged Clebsch-Gordan tables (first order only), tiles, barriers and schedules,
+// plus the 1 KB alignment slack.
+template <bool SO> constexpr size_t smem_bytes() {
+  constexpr int NST = SO ? SO_STAGES : STAGES;
+  return 2 * (size_t)A_IMAGE_BYTES + (size_t)NST * STAGE_BYTES +
+         (2 * (SO ? WG_BUF_SO : WG_BUF) + 2 * BM * 9 + (SO ? 0 : MAX_PATHS * MTAB)) * 4 + MAX_TILES * 8 * 4 +
+         (NST + 4) * sizeof(uint64_t) + (4 * SCHED_WORDS + NST) * 4 + 1024;
+}
+
+// SO = false: the first-order kernel (d_in, d_out <= 3, kinds 0-5, <= 16 paths).  SO = true: the second-order one (d_in,
+// d_out <= 5, kinds 0-7, <= 32 paths); a (10, 5) tile (kind 6) would need 100 partial sums beside the 96 accumulator
+// registers, so it contracts its block in two slices, components 0-2 then 3-4, from the same accumulator tile and scatters
+// each slice at the end of the tile (not of the output irrep): 60 and 40 partial sums, the budget of kind 1.
+template <bool SO>
+__device__ __forceinline__ void fused_conv_body(const FusedParams& p) {
+  constexpr int NST = SO ? SO_STAGES : STAGES;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   unsigned char* sA = smem;                                      // [2 warpgroups][MAX_KA x 8 KB]
   unsigned char* sB = smem + 2 * (size_t)A_IMAGE_BYTES;          // ring of B stages
-  float* sBuf = reinterpret_cast<float*>(sB + STAGES * STAGE_BYTES);   // [2 warpgroups][WG_BUF]: z rows / scatter staging
-  float* sY = sBuf + 2 * WG_BUF;                                 // [2][64][9] edge_weight * spherical harmonics per edge
-  float* sMtab = sY + 2 * BM * 9;                                // [MAX_PATHS][48]
-  int* sTiles = reinterpret_cast<int*>(sMtab + MAX_PATHS * MTAB);   // [MAX_TILES][8]
+  float* sBuf = reinterpret_cast<float*>(sB + NST * STAGE_BYTES);      // [2 warpgroups][WG_BUF]: z rows / scatter staging
+  float* sY = sBuf + 2 * (SO ? WG_BUF_SO : WG_BUF);              // [2][64][9] edge_weight * spherical harmonics per edge
+  float* sMtab = sY + 2 * BM * 9;                                // [MAX_PATHS][48] (first order)
+  int* sTiles = reinterpret_cast<int*>(sMtab + (SO ? 0 : MAX_PATHS * MTAB));   // [MAX_TILES][8]
   uint64_t* full = reinterpret_cast<uint64_t*>(sTiles + MAX_TILES * 8);   // B stage s has landed (TMA complete_tx)
-  unsigned long long* sDbg = reinterpret_cast<unsigned long long*>(full + STAGES);   // [2][2] debug clocks per warpgroup
+  unsigned long long* sDbg = reinterpret_cast<unsigned long long*>(full + NST);   // [2][2] debug clocks per warpgroup
   uint32_t* sOps = reinterpret_cast<uint32_t*>(sDbg + 4);       // [2 warpgroups][W1', W2'][SCHED_WORDS] MMA schedules
-  uint32_t* sRel = sOps + 4 * SCHED_WORDS;                       // [STAGES] releases of each stage
+  uint32_t* sRel = sOps + 4 * SCHED_WORDS;                       // [NST] releases of each stage
 
   const int tid = threadIdx.x;
   const int S1 = p.K1p >> 4, S2 = p.Hp >> 4;
   for (int i = tid; i < p.n_tiles * 8; i += THREADS) sTiles[i] = p.tiles[i];
-  for (int i = tid; i < p.n_paths * MTAB; i += THREADS) sMtab[i] = p.mtab[i];
+  if constexpr (!SO)
+    for (int i = tid; i < p.n_paths * MTAB; i += THREADS) sMtab[i] = p.mtab[i];
   if (tid % 32 == 0 && tid < 128) {
     const int wg = tid >> 6, which = (tid >> 5) & 1;
     build_ops(sOps + (2 * wg + which) * SCHED_WORDS, which ? S2 : S1, gmma_desc_lo(smem_u32(sA + wg * A_IMAGE_BYTES)));
   }
-  if (tid < STAGES) sRel[tid] = 0u;
+  if (tid < NST) sRel[tid] = 0u;
   if (tid < 4) sDbg[tid] = 0ull;
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) mbar_init(&full[s], 1);
+    for (int s = 0; s < NST; ++s) mbar_init(&full[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -549,13 +616,13 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
     atomicAdd(p.dbg + 26, 0ull - g0);
   }
 
-  Stream st;
+  Stream<NST> st;
   st.sB = sB; st.full = full; st.rel = sRel; st.tiles = sTiles; st.n1 = n1;
   st.per_unit = p.n_kb1 + p.n_tiles * p.n_kb;
   st.len = (uint32_t)(my_units * st.per_unit);
   // the ring runs ahead across edge tiles: the next tile's W1' blocks are requested while this one is contracted
   if (tid == 0)
-    for (int i = 0; i < STAGES; ++i) st.issue(p, (uint32_t)i);
+    for (int i = 0; i < NST; ++i) st.issue(p, (uint32_t)i);
 
   // Warpgroup g owns edges 64 g .. 64 g + 63 of every 128-edge tile and does all of their work; the two warpgroups meet
   // only at the stages of the shared B stream.
@@ -564,9 +631,11 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
   const int r0 = 16 * w4 + (lane >> 2);                          // this thread's accumulator rows (edges) r0, r0 + 8
   const int rb = r0 + 8 * (q >> 1), ub = 8 * (q & 1);            // its z rows: edge rb, tile rows ub .. ub + 7
   unsigned char* sAg = sA + (size_t)g * A_IMAGE_BYTES;
-  float* buf = sBuf + g * WG_BUF;
+  float* buf = sBuf + g * (SO ? WG_BUF_SO : WG_BUF);
   float* zrow = buf + rb * ZLD;
   const float* zcon = buf + r0 * ZLD;
+  float* zrowb = buf + 64 * ZLD + rb * ZLDB;                     // SO: components 3, 4
+  const float* zconb = buf + 64 * ZLD + r0 * ZLDB;
   unsigned long long* dwait = (p.dbg && t == 0) ? sDbg + 2 * g : nullptr;
   const uint32_t* ops1 = sOps + 2 * g * SCHED_WORDS;
   const uint32_t* ops2 = ops1 + SCHED_WORDS;
@@ -607,8 +676,8 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
     const uint32_t head_mask = __ballot_sync(0xffffffffu, lane == 0 || key_up != dst_s || !vs);
 
     const float* xrow = p.x + (long long)src_b * p.ld_x;
-    float xn[XN], M[9], acc[NACC_MAX];
-    prefetch_tile(xrow, sTiles, ub, p.x_vec2, xn);
+    float xn[SO ? 1 : XN], M[SO ? 25 : 9], acc[NACC_MAX];
+    if constexpr (!SO) prefetch_tile(xrow, sTiles, ub, p.x_vec2, xn);
     Acc d;
     mma_product(d, p, st, ops1, p.n_kb1, mc, bar, t, dwait);
     store_hidden(d, p, sAg, t, bar);
@@ -621,7 +690,20 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
       }
       // M[i,k] = edge_weight * sum_j coef*C[i,j,k] * Y[sh_off + j]  (at most 3x3 for the supported paths; row-major,
       // stride 3), rebuilt only when the tile belongs to another path than its predecessor: dense table, fully unrolled
-      if (flags & 4) {
+      if (SO && (flags & 4)) {    // [5][5] from the [5][5][5] table in global memory (L1), stride 5
+        const float* T = p.mtab + tt[7] * SO_MTAB;
+        const int sh_off = (flags >> 8) & 0xff;
+        float yb[5];
+#pragma unroll
+        for (int j = 0; j < 5; ++j) yb[j] = Y[min(sh_off + j, 8)];
+#pragma unroll
+        for (int ik = 0; ik < 25; ++ik) {
+          float a = 0.f;
+#pragma unroll
+          for (int j = 0; j < 5; ++j) a = fmaf(__ldg(T + ik * 5 + j), yb[j], a);
+          M[ik] = a;
+        }
+      } else if (flags & 4) {
         const float* T = sMtab + tt[7] * MTAB;
         const int sh_off = (flags >> 8) & 0xff;
         float yb[5];
@@ -636,9 +718,20 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
         }
       }
       // z of this tile from the node values prefetched one tile ahead; then the next tile's values are requested, so that
-      // their latency hides behind this tile's MMAs
-      __syncwarp();                              // the quad has read the previous tile's z rows
-      switch (kind) {
+      // their latency hides behind this tile's MMAs (SO: read by build_z_so itself)
+      __syncwarp();                             // the quad has read the previous tile's z rows
+      if constexpr (SO) {
+        const float* xs = xrow + tt[2] + ub * d_in;
+        const int nr = min(max(tt[3] - ub, 0), 8);
+        switch (kind) {
+          case 0: build_z_so<1, 4>(xs, nr, d_in, M, zrow, zrowb, ub); break;
+          case 1: case 3: build_z_so<3, 16>(xs, nr, d_in, M, zrow, zrowb, ub); break;
+          case 2: build_z_so<1, 8>(xs, nr, d_in, M, zrow, zrowb, ub); break;
+          case 4: case 5: build_z_so<1, 16>(xs, nr, d_in, M, zrow, zrowb, ub); break;
+          case 6: case 7: build_z_so<5, 16>(xs, nr, d_in, M, zrow, zrowb, ub); break;
+          default: __trap();   // unreachable: FusedPlan writes kinds 0-7 only (fused.py:CONSUMER_KINDS)
+        }
+      } else switch (kind) {
         case 0: build_z<1, 4>(xn, d_in, M, zrow, ub); break;
         case 1: build_z<3, 16>(xn, d_in, M, zrow, ub); break;
         case 2: build_z<1, 8>(xn, d_in, M, zrow, ub); break;
@@ -647,28 +740,63 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
         default: __trap();     // unreachable: FusedPlan writes kinds 0-5 only (fused.py:CONSUMER_KINDS)
       }
       __syncwarp();
-      if (ti + 1 < p.n_tiles) prefetch_tile(xrow, tt + 8, ub, p.x_vec2, xn);
+      if (!SO && ti + 1 < p.n_tiles) prefetch_tile(xrow, tt + 8, ub, p.x_vec2, xn);
       mma_product(d, p, st, ops2, p.n_kb, mc, bar, t, dwait);
       const long long c0 = dwait ? clock64() : 0;
       const int nch = tt[1] >> 5;
-      switch (kind) {
-        case 0: contract<48, 1, 4>(d, zcon, nch, q, acc); break;
-        case 1: contract<10, 3, 16>(d, zcon, nch, q, acc); break;
-        case 2: contract<16, 1, 8>(d, zcon, nch, q, acc); break;
-        case 3: contract<4, 3, 16>(d, zcon, nch, q, acc); break;
-        case 4: contract<10, 1, 16>(d, zcon, nch, q, acc); break;
-        case 5: contract<4, 1, 16>(d, zcon, nch, q, acc); break;
-        default: __trap();
-      }
-      if (flags & 2) {
+      if constexpr (SO) {
         switch (kind) {
-          case 0: flush<48, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-          case 1: flush<10, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-          case 2: flush<16, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-          case 3: flush<4, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-          case 4: flush<10, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-          case 5: flush<4, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+          case 0: contract<48, 1, 4>(d, zcon, nch, q, acc); break;
+          case 1: contract<10, 3, 16>(d, zcon, nch, q, acc); break;
+          case 2: contract<16, 1, 8>(d, zcon, nch, q, acc); break;
+          case 3: contract<4, 3, 16>(d, zcon, nch, q, acc); break;
+          case 4: contract<10, 1, 16>(d, zcon, nch, q, acc); break;
+          case 5: contract<4, 1, 16>(d, zcon, nch, q, acc); break;
+          case 6:                  // (10, 5): components 0-2, scattered, then 3-4 from the same accumulator tile
+#pragma unroll
+            for (int i = 0; i < NACC_MAX; ++i) acc[i] = 0.f;
+            contract<10, 3, 16>(d, zcon, nch, q, acc);
+            flush<10, 3, 5, 0>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar);
+#pragma unroll
+            for (int i = 0; i < NACC_MAX; ++i) acc[i] = 0.f;
+            contract<10, 2, 16, 3>(d, zcon, nch, q, acc, zconb);
+            flush<10, 2, 5, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar);
+            break;
+          case 7: contract<4, 5, 16>(d, zcon, nch, q, acc, zconb); break;
           default: __trap();
+        }
+        if ((flags & 2) && kind != 6) {
+          switch (kind) {
+            case 0: flush<48, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 1: flush<10, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 2: flush<16, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 3: flush<4, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 4: flush<10, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 5: flush<4, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 7: flush<4, 5>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            default: __trap();
+          }
+        }
+      } else {
+        switch (kind) {
+          case 0: contract<48, 1, 4>(d, zcon, nch, q, acc); break;
+          case 1: contract<10, 3, 16>(d, zcon, nch, q, acc); break;
+          case 2: contract<16, 1, 8>(d, zcon, nch, q, acc); break;
+          case 3: contract<4, 3, 16>(d, zcon, nch, q, acc); break;
+          case 4: contract<10, 1, 16>(d, zcon, nch, q, acc); break;
+          case 5: contract<4, 1, 16>(d, zcon, nch, q, acc); break;
+          default: __trap();
+        }
+        if (flags & 2) {
+          switch (kind) {
+            case 0: flush<48, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 1: flush<10, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 2: flush<16, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 3: flush<4, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 4: flush<10, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 5: flush<4, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            default: __trap();
+          }
         }
       }
       if (dwait) dwait[1] += (unsigned long long)(clock64() - c0);
@@ -694,10 +822,13 @@ __global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParam
   }
 }
 
+__global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParams p) { fused_conv_body<false>(p); }
+__global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel_so(const FusedParams p) { fused_conv_body<true>(p); }
+
 // per-device state: debug counters and the one-time opt-in to > 48 KB of dynamic shared memory
 constexpr int MAX_DEVICES = 64;
 struct DeviceState {
-  bool attr_done = false;
+  bool attr_done = false, attr_done_so = false;
   bool dbg_init = false;
   unsigned long long* dbg = nullptr;
 };
@@ -717,6 +848,7 @@ unsigned long long* fused_debug_buffer(int dev) {
 
 }  // namespace
 
+
 // Diagnostics (DDB200_FUSED_DEBUG=1 only): copies the 32 clock counters of the fused kernel (current device) to `out` and
 // clears them.  [11] clocks spent per 128-edge tile by warpgroup 0 (summed over tiles), [12] 64-edge units (two per
 // 128-edge tile), [13] clocks the warpgroups spent waiting for a B stage to land, [14] clocks they spent contracting and
@@ -733,12 +865,16 @@ extern "C" int ddb200_fused_debug_read(uint64_t* out) {
   return (int)e;
 }
 
-extern "C" int ddb200_fused_conv(const ddb200_fused_args* a, void* stream) {
+namespace {
+
+template <bool SO>
+int fused_conv_launch(const ddb200_fused_args* a, void* stream) {
   if (!a || !a->edge_attr || !a->w1_images || !a->w2_images || !a->tiles || !a->mtab || !a->x || !a->edge_vec || !a->sum ||
       !a->tgt || !a->src || a->n_edges < 0 || a->ne <= 0 || a->ns < 0 || a->hidden <= 0 || a->n_tiles <= 0 || a->d_out <= 0)
     return DDB200_EINVAL;
   if (a->ns > 0 && (!a->node || a->ld_node < a->ns)) return DDB200_EINVAL;
-  if (a->n_tiles > MAX_TILES || a->n_paths <= 0 || a->n_paths > MAX_PATHS || a->sh_lmax < 0 || a->sh_lmax > 2)
+  if (a->n_tiles > MAX_TILES || a->n_paths <= 0 || a->n_paths > (SO ? SO_MAX_PATHS : MAX_PATHS) || a->sh_lmax < 0 ||
+      a->sh_lmax > 2)
     return DDB200_EINVAL;
   if ((a->ea_add == nullptr) != (a->ea_add_idx == nullptr)) return DDB200_EINVAL;
   const int K1 = a->ne + 2 * a->ns, H = a->hidden;
@@ -769,16 +905,24 @@ extern "C" int ddb200_fused_conv(const ddb200_fused_args* a, void* stream) {
   p.dbg = fused_debug_buffer(dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long n_mtiles = (a->n_edges + CTA_EDGES - 1) / CTA_EDGES;
-  const size_t fixed = (2 * WG_BUF + 2 * BM * 9 + MAX_PATHS * MTAB) * 4 + MAX_TILES * 8 * 4 + (STAGES + 4) * sizeof(uint64_t) +
-                       (4 * SCHED_WORDS + STAGES) * 4 + 1024;
-  const size_t smem = 2 * (size_t)A_IMAGE_BYTES + (size_t)STAGES * STAGE_BYTES + fixed;
+  const size_t smem = smem_bytes<SO>();
   if (smem > 227 * 1024) return DDB200_ESMEM;
-  if (!g_dev[dev].attr_done) {      // the opt-in is a per-device attribute
-    const cudaError_t e = cudaFuncSetAttribute(fused_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  auto kernel = SO ? fused_conv_kernel_so : fused_conv_kernel;
+  bool& attr_done = SO ? g_dev[dev].attr_done_so : g_dev[dev].attr_done;
+  if (!attr_done) {                 // the opt-in is a per-device, per-kernel attribute
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
-    g_dev[dev].attr_done = true;
+    attr_done = true;
   }
   const unsigned grid = (unsigned)(n_mtiles < sms ? n_mtiles : sms);
-  fused_conv_kernel<<<grid, THREADS, smem, (cudaStream_t)stream>>>(p);
+  kernel<<<grid, THREADS, smem, (cudaStream_t)stream>>>(p);
   return (int)cudaGetLastError();
 }
+
+}  // namespace
+
+extern "C" int ddb200_fused_conv(const ddb200_fused_args* a, void* stream) { return fused_conv_launch<false>(a, stream); }
+
+// The second-order instantiation: plans with a 5-component input or output block (fused.py:FusedPlan.second_order); the
+// Clebsch-Gordan tables are [n_paths][5][5][5] padded to 128 floats.
+extern "C" int ddb200_fused_conv_so(const ddb200_fused_args* a, void* stream) { return fused_conv_launch<true>(a, stream); }

@@ -11,11 +11,19 @@ whole rows ``u`` of one path block ``[mul_in, mul_out]``:
     (16, 1): 8 x 16 = 128                                            (4, 3): 16 x 4 = 64
     (10, 1): 16 x 10 = 160                                           (4, 1): 16 x 4 = 64
 
-(the two ``(nv, 1)`` kinds are the ``nv x0o`` blocks that ``reduce_pseudoscalars`` gives layers 2 and up)
+    (10, 5): 16 x 10 = 160                                           (4, 5): 16 x 4 = 64
+
+(the two ``(nv, 1)`` kinds are the ``nv x0o`` blocks that ``reduce_pseudoscalars`` gives layers 2 and up; the two
+``(nv, 5)`` kinds are the ``nv x2e`` / ``nv x2o`` blocks of ``use_second_order_repr``)
+
+A plan with a 5-component input or output block (``use_second_order_repr``) runs on the kernel's second-order
+instantiation (``ddb200_fused_conv_so``): up to 32 paths, dense [5][5][5] tables, and each (10, 5) tile scattered at its
+own end in two slices (components 0-2, 3-4), because 100 partial sums per thread would not fit beside the accumulators.
 
 so that a consumer thread (one edge = one accumulator row) knows at compile time which register of its accumulator every
 accumulator column feeds.  This module builds, from a ``TpTable`` and the radial MLP's second Linear:
-  * the tile table (int32 [T, 8]) and one dense Clebsch-Gordan table per path ([3][3][5] floats: coef * C[i, j, k]),
+  * the tile table (int32 [T, 8]) and one dense Clebsch-Gordan table per path ([3][3][5] floats: coef * C[i, j, k];
+    second order: [5][5][5]),
   * the pre-split, pre-swizzled bf16 operand images of W2 per tile (rows permuted into tile order, zero padded), with the
     bias folded in as two extra K columns (hi, lo) that multiply constant-one columns of the activation operand.
     Image columns are [hi | lo | bias] in 16-column-aligned sections; the kernel's activation image is [hi | lo | 1 1] and
@@ -37,10 +45,14 @@ from .radial import BK, BN
 from .tp_table import TpTable
 
 # (mul_out, d_out) -> (consumer kind id, rows per tile)
-CONSUMER_KINDS = {(48, 1): (0, 4), (10, 3): (1, 16), (16, 1): (2, 8), (4, 3): (3, 16), (10, 1): (4, 16), (4, 1): (5, 16)}
+CONSUMER_KINDS = {(48, 1): (0, 4), (10, 3): (1, 16), (16, 1): (2, 8), (4, 3): (3, 16), (10, 1): (4, 16), (4, 1): (5, 16),
+                  (10, 5): (6, 16), (4, 5): (7, 16)}
 MAX_K = 144          # widest radial-MLP input / hidden layer (16-column sections: 2 * 144 + 16 = 304 -> 5 k-blocks of 64)
 MAX_TILES = 128      # tile table capacity of the kernel (csrc/fused_conv.cu)
 MTAB = 48            # floats per path in the dense Clebsch-Gordan table: [3][3][5] padded
+MAX_PATHS = 16
+MTAB_SO = 128        # second-order instantiation: [5][5][5] padded
+MAX_PATHS_SO = 32
 ENABLED = os.environ.get('DDB200_FUSED_CONV', '1') != '0'
 
 
@@ -48,17 +60,22 @@ def _pad16(k: int) -> int:
     return (k + 15) // 16 * 16
 
 
+def second_order(table: TpTable) -> bool:
+    """True when the layer has a 5-component input or output block: it runs on the second-order instantiation."""
+    return any(p.l_in == 2 or p.l_out == 2 for p in table.paths)
+
+
 def supported(table: TpTable, hidden: int, k1: int) -> bool:
     if table.sh_lmax < 0 or table.sh_lmax > 2:
         return False
     if _pad16(hidden) > MAX_K or _pad16(k1) > MAX_K:
         return False
-    if len(table.paths) > 16:
+    if len(table.paths) > (MAX_PATHS_SO if second_order(table) else MAX_PATHS):
         return False
     for p in table.paths:
         if (p.mul_out, 2 * p.l_out + 1) not in CONSUMER_KINDS:
             return False
-        if (2 * p.l_in + 1) not in (1, 3) or p.l_sh > 2:
+        if (2 * p.l_in + 1) not in (1, 3, 5) or p.l_sh > 2:
             return False
     n_tiles = sum(-(-p.mul_in // CONSUMER_KINDS[(p.mul_out, 2 * p.l_out + 1)][1]) for p in table.paths)
     return n_tiles <= MAX_TILES
@@ -95,16 +112,19 @@ class FusedPlan:
         H, K1 = w1.shape
         assert supported(table, H, K1)
         self.table, self.hidden, self.k1 = table, H, K1
+        self.second_order = second_order(table)
         paths = sorted(table.paths, key=lambda p: (p.i_out, p.w_ref_off))
         tiles, row_src = [], []
-        # dense Clebsch-Gordan table per path: mtab[path][i][k][j] = coef * C[i, j, k]   (i, k < 3, j < 5; zero padded)
-        mtab = np.zeros((len(paths), MTAB), dtype=np.float32)
+        # dense Clebsch-Gordan table per path: mtab[path][i][k][j] = coef * C[i, j, k]   (i, k < D, j < 5; zero padded),
+        # D = 3 (first order) or 5 (second order)
+        D = 5 if self.second_order else 3
+        mtab = np.zeros((len(paths), MTAB_SO if self.second_order else MTAB), dtype=np.float32)
         for pi, p in enumerate(paths):
             C = real_cg(p.l_in, p.l_sh, p.l_out)
             d_in, d_sh, d_out = C.shape
-            blk = np.zeros((3, 3, 5))
+            blk = np.zeros((D, D, 5))
             blk[:d_in, :d_out, :d_sh] = p.coef * np.transpose(C, (0, 2, 1))
-            mtab[pi, :45] = blk.reshape(-1)
+            mtab[pi, :D * D * 5] = blk.reshape(-1)
         group_prev = None
         path_prev = None
         for pi, p in enumerate(paths):
@@ -210,7 +230,8 @@ def fused_conv(plan: FusedPlan, edge_attr, node, ns, tgt32, src32, x, edge_vec, 
     if prof:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-    rc = _lib.lib().ddb200_fused_conv(C.byref(a), _stream())
+    launch = _lib.lib().ddb200_fused_conv_so if plan.second_order else _lib.lib().ddb200_fused_conv
+    rc = launch(C.byref(a), _stream())
     if prof:
         e1.record()
         n_live = int(n_edges_dev.item()) if n_edges_dev is not None else E      # profiling replay only (host sync)

@@ -288,7 +288,7 @@ class TensorProductConvLayer(nn.Module):
                 prepared.append(None)
             s = e
         return self._run(x, prepared, fcs, from_vec, ew_scalar, n_out, reduce, gather_scalars, scale, shift,
-                         residual=residual).to(_dtype)
+                         residual=residual, second_order=False).to(_dtype)
 
     @torch.no_grad()
     def forward_groups(self, node_attr, groups, out_nodes=None, reduce='mean', gather_scalars=0, init=None):
@@ -332,7 +332,8 @@ class TensorProductConvLayer(nn.Module):
 
     def fused_capable(self, k_edge, gather_scalars):
         """True if every radial MLP of this layer runs on the fully fused kernel for ``k_edge`` per-edge attribute columns
-        (+ 2 x ``gather_scalars`` node scalars) with in-kernel spherical harmonics."""
+        (+ 2 x ``gather_scalars`` node scalars) with in-kernel spherical harmonics, through ``forward_groups`` (layers with
+        l = 2 blocks: through the grouped entry points only, see ``_run``)."""
         if not self.tp.vec_capable:
             return False
         table = self.tp.table_vec
@@ -341,7 +342,11 @@ class TensorProductConvLayer(nn.Module):
         return all(fused.ENABLED and self._fusable(fc, k_in) and fused.supported(table, fc[0].out_features, k_in) for fc in fcs)
 
     def _run(self, x, prepared, fcs, from_vec, ew_scalar, n_out, reduce, gather_scalars, scale, shift, residual=None,
-             init=None, finalize=True, swap_gathered=False):
+             init=None, finalize=True, swap_gathered=False, second_order=True):
+        """``second_order``: layers with l = 2 blocks may take the fused kernel's second-order instantiation.  Only the
+        grouped entry points (``forward_groups`` / ``accumulate_group``, the models' convolution stacks) allow it; the
+        reference-signature ``forward`` keeps such layers on the streaming kernel, as it ran them before that
+        instantiation existed."""
         handle = self.tp.handle(from_vec)
         table = handle.table
         if init is not None:
@@ -359,7 +364,8 @@ class TensorProductConvLayer(nn.Module):
             n_e = tgt32.shape[0]
             k_in = ea.shape[1] + 2 * gather_scalars
             plan = self._fused_plan(fc, table, k_in, gather_scalars if swap_gathered else 0) \
-                if (from_vec and ew_scalar == 1.0 and (n_e >= 64 or extras is not None)) else None
+                if (from_vec and ew_scalar == 1.0 and (n_e >= 64 or extras is not None)
+                    and (second_order or not fused.second_order(table))) else None
             if swap_gathered and plan is None:
                 raise RuntimeError("swapped node scalars (swap_gathered) need a fused-kernel layer shape "
                                    "(TensorProductConvLayer.fused_capable)")

@@ -211,8 +211,8 @@ int ddb200_radial_mlp(const float* edge_attr, int64_t ld_ea, int ne, const float
  * per-complex sigma-embedding term of models/cg_model.py:298-301 without materialising edge_attr + sigma per step.
  * w1_images / w2_images / tiles / mtab: the plan built by diffdock_b200/fused.py (operand images [hi | lo | bias] with
  * 16-column-aligned sections, N tiles = whole rows of one path block, dense Clebsch-Gordan tables [path][3][3][5] padded to
- * 48 floats).  Supported shapes: (mul_out, 2l_out+1) in {(48,1),(10,3),(16,1),(4,3)}, l_in <= 1, spherical harmonics from
- * edge vectors (sh_lmax <= 2), ne + 2 ns <= 144, hidden <= 144.
+ * 48 floats).  Supported shapes: (mul_out, 2l_out+1) in {(48,1),(10,3),(16,1),(4,3),(10,1),(4,1)}, l_in <= 1, at most
+ * 16 paths, spherical harmonics from edge vectors (sh_lmax <= 2), ne + 2 ns <= 144, hidden <= 144.
  * Any base pointer and row stride is accepted.  The rows of a are read with 16-byte loads when ne % 8 == 0, ns % 8 == 0,
  * ld_ea % 4 == 0, edge_attr 16-byte aligned, and (ns > 0) ld_node % 4 == 0 and node 16-byte aligned, and (ea_add given)
  * ea_add 16-byte aligned; otherwise element by element.  x is read with 8-byte loads when x_pairs_ok, ld_x is even and x
@@ -239,6 +239,10 @@ typedef struct ddb200_fused_args {
 } ddb200_fused_args;
 
 int ddb200_fused_conv(const ddb200_fused_args* args, void* stream);
+/* Second-order instantiation (node irreps with l = 2 blocks, use_second_order_repr): same arguments, additionally
+ * (mul_out, 2l_out+1) in {(10,5),(4,5)} and l_in <= 2, at most 32 paths, mtab = [n_paths][5][5][5] padded to 128 floats;
+ * x is read element by element (x_pairs_ok is ignored). */
+int ddb200_fused_conv_so(const ddb200_fused_args* args, void* stream);
 /* Execution: one CTA per SM, persistent over tiles of 64 edges; one warpgroup issues wgmma, one contracts. */
 
 /* Diagnostics, no reference counterpart: with DDB200_FUSED_DEBUG=1 in the environment the fused kernel accumulates clock
