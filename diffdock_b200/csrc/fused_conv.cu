@@ -6,6 +6,7 @@
 //     A0' = split-bf16([edge_attr (+ per-graph term) | node[tgt,:ns] | node[src,:ns]])   the warpgroup's own image in shared
 //                                      memory (128B swizzle)
 //     H   = relu(A0' x W1'^T)          wgmma -> registers -> A' image (bias folded via two constant-one columns)
+//     H   = relu(A' x Wh'^T)           for every extra H x H hidden layer (tp_weights_layers > 2), in place over A'
 //     for every N tile (whole rows u of one path block [mul_in, mul_out], <= 192 columns):
 //        z_e[u,k] = sum_i x[src_e][u,i] M_e[i,k],  M_e = edge_weight * coef * C . Y(vec_e)   built by each quad of threads
 //                                      for its two edges in a per-warpgroup shared-memory buffer
@@ -114,6 +115,7 @@ struct FusedParams {
   float vec_sign;
   const __nv_bfloat16* w1img; int K1, K1p, n_kb1, H, Hp, n_kb;
   const __nv_bfloat16* w2img;                        // [n_tiles][n_kb][256][64]
+  const __nv_bfloat16* whimg; int n_hidden;          // [n_hidden][n_kb][256][64]: extra H x H hidden layers, in order
   const int* tiles; int n_tiles;                     // [n_tiles][8]: kind, N_mma, x_off, rows, d_in, out_off, flags | sh_off << 8, path
   const float* mtab; int n_paths;                    // [n_paths][48]: coef * C[i, j, k] as [i][k][j], i,k < 3, j < 5
   const float* x; long long ld_x; int x_vec2;        // node irreps gathered by src
@@ -352,22 +354,26 @@ __device__ __forceinline__ void build_ops(uint32_t* ops, int S, uint32_t a_lo0) 
   }
 }
 
-// B stream of a CTA: per edge tile the W1' k-blocks, then every N tile's W2' k-blocks; item i goes to stage i % NST and
-// is read by both warpgroups
+// B stream of a CTA: per edge tile the W1' k-blocks, then the Wh' k-blocks of every extra hidden layer in order, then
+// every N tile's W2' k-blocks; item i goes to stage i % NST and is read by both warpgroups
 template <int NST> struct Stream {
   unsigned char* sB; uint64_t* full; uint32_t* rel; const int* tiles;
   int n1, per_unit; uint32_t len;
   __device__ __forceinline__ void issue(const FusedParams& p, uint32_t i) const {
     if (i >= len) return;
     const int j = (int)(i % (uint32_t)per_unit);
+    const int jh = j - p.n_kb1, j2 = jh - p.n_hidden * p.n_kb;
     const unsigned char* src;
     uint32_t bytes;
     if (j < p.n_kb1) {
       src = reinterpret_cast<const unsigned char*>(p.w1img) + (size_t)j * B_IMAGE_BYTES;
       bytes = (uint32_t)n1 * 128u;
-    } else {                    // image (t, kb) of the W2' set lies at (t * n_kb + kb) = j - n_kb1
-      src = reinterpret_cast<const unsigned char*>(p.w2img) + (size_t)(j - p.n_kb1) * B_IMAGE_BYTES;
-      bytes = (uint32_t)tiles[((j - p.n_kb1) / p.n_kb) * 8 + 1] * 128u;
+    } else if (j2 < 0) {        // image (l, kb) of the Wh' set lies at (l * n_kb + kb) = jh; its H rows as for W1'
+      src = reinterpret_cast<const unsigned char*>(p.whimg) + (size_t)jh * B_IMAGE_BYTES;
+      bytes = (uint32_t)n1 * 128u;
+    } else {                    // image (t, kb) of the W2' set lies at (t * n_kb + kb) = j2
+      src = reinterpret_cast<const unsigned char*>(p.w2img) + (size_t)j2 * B_IMAGE_BYTES;
+      bytes = (uint32_t)tiles[(j2 / p.n_kb) * 8 + 1] * 128u;
     }
     const uint32_t s = i % NST;
     bulk_load(sB + (size_t)s * STAGE_BYTES, src, bytes, &full[s]);
@@ -618,7 +624,7 @@ __device__ __forceinline__ void fused_conv_body(const FusedParams& p) {
 
   Stream<NST> st;
   st.sB = sB; st.full = full; st.rel = sRel; st.tiles = sTiles; st.n1 = n1;
-  st.per_unit = p.n_kb1 + p.n_tiles * p.n_kb;
+  st.per_unit = p.n_kb1 + p.n_hidden * p.n_kb + p.n_tiles * p.n_kb;
   st.len = (uint32_t)(my_units * st.per_unit);
   // the ring runs ahead across edge tiles: the next tile's W1' blocks are requested while this one is contracted
   if (tid == 0)
@@ -679,8 +685,16 @@ __device__ __forceinline__ void fused_conv_body(const FusedParams& p) {
     float xn[SO ? 1 : XN], M[SO ? 25 : 9], acc[NACC_MAX];
     if constexpr (!SO) prefetch_tile(xrow, sTiles, ub, p.x_vec2, xn);
     Acc d;
-    mma_product(d, p, st, ops1, p.n_kb1, mc, bar, t, dwait);
-    store_hidden(d, p, sAg, t, bar);
+    // the hidden stack, one product loop: W1' from A0' (schedule ops1, n_kb1 k-blocks), then each extra H x H layer Wh'
+    // from the A' image (ops2, n_kb k-blocks, the geometry of the W2' products).  store_hidden writes each layer's ReLU
+    // over the image its product read: mma_product returns only once every group of the product is complete in all four
+    // warps (the release's barrier follows the last wait), and store_hidden fences to the async proxy and meets at the
+    // barrier before the next product reads the image.
+#pragma unroll 1
+    for (int l = 0; l <= p.n_hidden; ++l) {
+      mma_product(d, p, st, l ? ops2 : ops1, l ? p.n_kb : p.n_kb1, mc, bar, t, dwait);
+      store_hidden(d, p, sAg, t, bar);
+    }
     for (int ti = 0; ti < p.n_tiles; ++ti) {
       const int* tt = sTiles + ti * 8;
       const int kind = tt[0], d_in = tt[4], out_off = tt[5], flags = tt[6];
@@ -882,6 +896,8 @@ int fused_conv_launch(const ddb200_fused_args* a, void* stream) {
   const int n_kb = (2 * Hp + 16 + BK - 1) / BK, n_kb1 = (2 * K1p + 16 + BK - 1) / BK;
   if (n_kb > MAX_KB || n_kb1 > MAX_KB || H > MAX_N) return DDB200_EINVAL;
   if ((reinterpret_cast<uintptr_t>(a->w1_images) & 127) || (reinterpret_cast<uintptr_t>(a->w2_images) & 127)) return DDB200_EINVAL;
+  if (a->n_hidden < 0 || (a->n_hidden > 0 && (!a->wh_images || (reinterpret_cast<uintptr_t>(a->wh_images) & 127))))
+    return DDB200_EINVAL;
   if (a->n_edges == 0) return 0;
   FusedParams p = {};
   p.ea = a->edge_attr; p.ld_ea = a->ld_ea; p.ne = a->ne; p.node = a->node; p.ld_node = a->ld_node; p.ns = a->ns;
@@ -895,6 +911,7 @@ int fused_conv_launch(const ddb200_fused_args* a, void* stream) {
   p.w1img = reinterpret_cast<const __nv_bfloat16*>(a->w1_images); p.K1 = K1; p.K1p = K1p; p.n_kb1 = n_kb1;
   p.H = H; p.Hp = Hp; p.n_kb = n_kb;
   p.w2img = reinterpret_cast<const __nv_bfloat16*>(a->w2_images); p.tiles = a->tiles; p.n_tiles = a->n_tiles;
+  p.whimg = reinterpret_cast<const __nv_bfloat16*>(a->wh_images); p.n_hidden = a->n_hidden;
   p.mtab = a->mtab; p.n_paths = a->n_paths;
   p.x = a->x; p.ld_x = a->ld_x; p.x_vec2 = (a->x_pairs_ok && (a->ld_x & 1) == 0 && (reinterpret_cast<uintptr_t>(a->x) & 7) == 0) ? 1 : 0;
   p.vec = a->edge_vec; p.ew = a->edge_weight; p.lmax = a->sh_lmax; p.sum = a->sum; p.d_out = a->d_out; p.cnt = a->cnt;

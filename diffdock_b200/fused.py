@@ -20,6 +20,9 @@ A plan with a 5-component input or output block (``use_second_order_repr``) runs
 instantiation (``ddb200_fused_conv_so``): up to 32 paths, dense [5][5][5] tables, and each (10, 5) tile scattered at its
 own end in two slices (components 0-2, 3-4), because 100 partial sums per thread would not fit beside the accumulators.
 
+A radial MLP built with ``tp_weights_layers`` > 2 passes its extra H x H hidden layers as ``FusedPlan(..., hidden=...)``:
+one operand image each, streamed between W1' and the W2' tiles and applied in place over the activation image.
+
 so that a consumer thread (one edge = one accumulator row) knows at compile time which register of its accumulator every
 accumulator column feeds.  This module builds, from a ``TpTable`` and the radial MLP's second Linear:
   * the tile table (int32 [T, 8]) and one dense Clebsch-Gordan table per path ([3][3][5] floats: coef * C[i, j, k];
@@ -106,12 +109,17 @@ def _split_images(w_rows: torch.Tensor, bias_rows: torch.Tensor, K: int):
 class FusedPlan:
     """Device-resident plan of one (layer, edge group)."""
 
-    def __init__(self, table: TpTable, w1: torch.Tensor, b1: torch.Tensor, w2_ref: torch.Tensor, b2_ref: torch.Tensor):
-        """w1 [H, K1], b1 [H]; w2_ref [weight_numel, H], b2_ref [weight_numel] in the REFERENCE weight-row order."""
+    def __init__(self, table: TpTable, w1: torch.Tensor, b1: torch.Tensor, w2_ref: torch.Tensor, b2_ref: torch.Tensor,
+                 hidden=()):
+        """w1 [H, K1], b1 [H]; w2_ref [weight_numel, H], b2_ref [weight_numel] in the REFERENCE weight-row order;
+        ``hidden``: the FCBlock's extra hidden layers (``tp_weights_layers - 2`` of them) in order, each ``(W [H, H], b [H])``,
+        applied as ReLU(h W^T + b) after the first layer."""
         dev = w2_ref.device
         H, K1 = w1.shape
         assert supported(table, H, K1)
+        assert all(tuple(w.shape) == (H, H) and tuple(b.shape) == (H,) for w, b in hidden)
         self.table, self.hidden, self.k1 = table, H, K1
+        self.n_hidden = len(hidden)
         self.second_order = second_order(table)
         paths = sorted(table.paths, key=lambda p: (p.i_out, p.w_ref_off))
         tiles, row_src = [], []
@@ -160,6 +168,14 @@ class FusedPlan:
         b1p = torch.zeros((1, BN), dtype=torch.float32, device=dev)
         w1p[0, :H], b1p[0, :H] = w1.detach().float(), b1.detach().float()
         self.w1_images = _split_images(w1p, b1p, K1)
+        # one N tile per extra hidden layer, streamed between W1' and the W2' tiles: [n_hidden, n_kb, 256, 8, 8]
+        self.wh_images = None
+        if hidden:
+            whp = torch.zeros((self.n_hidden, BN, H), dtype=torch.float32, device=dev)
+            bhp = torch.zeros((self.n_hidden, BN), dtype=torch.float32, device=dev)
+            for l, (w, b) in enumerate(hidden):
+                whp[l, :H], bhp[l, :H] = w.detach().float(), b.detach().float()
+            self.wh_images = _split_images(whp, bhp, H)
         self.tiles = torch.as_tensor(np.asarray(tiles, dtype=np.int32), device=dev).contiguous()
         self.mtab = torch.as_tensor(mtab, device=dev).contiguous()
         # 8-byte gathers of the node values are possible when every tile's offset and value count is even
@@ -167,9 +183,9 @@ class FusedPlan:
         # bf16 tensor-core FLOPs issued per 64-edge tile (split-bf16 x3 + bias step, 16-column steps; the kernel issues every
         # product 192 columns wide)
         s2, s1 = 3 * (_pad16(H) // 16) + 1, 3 * (_pad16(K1) // 16) + 1
-        self.mma_flops_per_tile = 2 * 64 * 16 * 192 * (s1 + len(tiles) * s2)
+        self.mma_flops_per_tile = 2 * 64 * 16 * 192 * (s1 + (self.n_hidden + len(tiles)) * s2)
         # algorithmic FLOPs per edge of the same work (fp32 radial MLP + tensor-product contraction, SURVEY 8(d))
-        self.alg_flops_per_edge = 2 * K1 * H + 2 * H * table.weight_numel + sum(
+        self.alg_flops_per_edge = 2 * K1 * H + self.n_hidden * 2 * H * H + 2 * H * table.weight_numel + sum(
             2 * p.mul_in * p.mul_out * (2 * p.l_out + 1) + 2 * p.mul_in * (2 * p.l_in + 1) * (2 * p.l_sh + 1) * (2 * p.l_out + 1)
             for p in table.paths)
 
@@ -185,7 +201,8 @@ class _Args(C.Structure):
                 ('x', C.c_void_p), ('ld_x', C.c_int64), ('x_pairs_ok', C.c_int32),
                 ('edge_vec', C.c_void_p), ('edge_weight', C.c_void_p), ('sh_lmax', C.c_int32),
                 ('n_edges', C.c_int64), ('n_edges_dev', C.c_void_p),
-                ('sum', C.c_void_p), ('d_out', C.c_int32), ('cnt', C.c_void_p)]
+                ('sum', C.c_void_p), ('d_out', C.c_int32), ('cnt', C.c_void_p),
+                ('wh_images', C.c_void_p), ('n_hidden', C.c_int32)]
 
 
 def _p(t):
@@ -225,7 +242,7 @@ def fused_conv(plan: FusedPlan, edge_attr, node, ns, tgt32, src32, x, edge_vec, 
               _p(tgt32), _p(src32), _p(edge_perm), _p(ea_add), _p(ea_add_idx) if ea_add is not None else None,
               float(vec_sign), _p(plan.w1_images), plan.hidden, _p(plan.w2_images), _p(plan.tiles), plan.n_tiles,
               _p(plan.mtab), plan.n_paths, _p(x), x.stride(0), plan.x_pairs_ok, _p(edge_vec), _p(edge_weight),
-              t.sh_lmax, E, _p(n_edges_dev), _p(sum_buf), t.d_out, _p(cnt_buf))
+              t.sh_lmax, E, _p(n_edges_dev), _p(sum_buf), t.d_out, _p(cnt_buf), _p(plan.wh_images), plan.n_hidden)
     prof = PROFILE.enabled
     if prof:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

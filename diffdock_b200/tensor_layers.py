@@ -184,22 +184,46 @@ class TensorProductConvLayer(nn.Module):
         """Plan of the fully fused kernel for this radial MLP, or None when the shapes are outside its templates.
         ``swap_ns`` > 0: the MLP was trained on ``[ea | node[src] | node[tgt]]`` (ns columns each) while the kernel assembles
         ``[ea | node[tgt] | node[src]]``, so the two node blocks of the first Linear's columns trade places in the plan."""
-        if not (fused.ENABLED and self._fusable(fc, k_in) and fused.supported(table, fc[0].out_features, k_in)):
+        if not (fused.ENABLED and self._fused_mlp(fc, k_in) and fused.supported(table, fc[0].out_features, k_in)):
             return None
-        l1, l2 = fc[0], fc[-1]
-        key = (l1.weight._version, l1.bias._version, l2.weight._version, l2.bias._version, l2.weight.device)
+        lins = [m for m in fc if isinstance(m, nn.Linear)]
+        l1, l2 = lins[0], lins[-1]
+        key = tuple(v for lin in lins for v in (lin.weight._version, lin.bias._version)) + (l2.weight.device,)
         hit = self._pcache.get((id(fc), swap_ns))
         if hit is None or hit[0] != key:
             w1 = l1.weight
             if swap_ns:
                 ne = k_in - 2 * swap_ns
                 w1 = torch.cat([w1[:, :ne], w1[:, ne + swap_ns:], w1[:, ne:ne + swap_ns]], 1)
-            hit = (key, fused.FusedPlan(table, w1, l1.bias, l2.weight, l2.bias))
+            hidden = [(lin.weight, lin.bias) for lin in lins[1:-1]]
+            hit = (key, fused.FusedPlan(table, w1, l1.bias, l2.weight, l2.bias, hidden=hidden))
             self._pcache[(id(fc), swap_ns)] = hit
         return hit[1]
 
     @staticmethod
+    def _fused_mlp(fc, k_in):
+        """True if the radial MLP ``fc`` can run inside the fully fused kernel: ``[Linear, ReLU, Dropout] x (L - 1) +
+        [Linear]`` (FCBlock with ``tp_weights_layers`` = L >= 2, ReLU), every hidden Linear H x H, H <= fused.MAX_K."""
+        mods = list(fc)
+        n = (len(mods) + 2) // 3
+        if not (radial.USE_TENSOR_CORES and n >= 2 and len(mods) == 3 * n - 2 and k_in <= radial.MAX_K):
+            return False
+        if not (isinstance(mods[0], nn.Linear) and isinstance(mods[-1], nn.Linear)):
+            return False
+        H = mods[0].out_features
+        if H > fused.MAX_K or mods[-1].in_features != H:
+            return False
+        for i in range(n - 1):
+            lin, act, drop = mods[3 * i:3 * i + 3]
+            if not (isinstance(lin, nn.Linear) and isinstance(act, nn.ReLU) and isinstance(drop, nn.Dropout)):
+                return False
+            if i > 0 and (lin.in_features, lin.out_features) != (H, H):
+                return False
+        return True
+
+    @staticmethod
     def _fusable(fc, k_in):
+        """The host-sized path's one-kernel radial MLP (``ddb200_radial_mlp``): two-layer FCBlocks only."""
         return (radial.USE_TENSOR_CORES and len(fc) == 4 and isinstance(fc[1], nn.ReLU) and isinstance(fc[0], nn.Linear)
                 and isinstance(fc[3], nn.Linear) and fc[0].out_features <= radial.MAX_K and k_in <= radial.MAX_K)
 
@@ -339,7 +363,8 @@ class TensorProductConvLayer(nn.Module):
         table = self.tp.table_vec
         fcs = [self.fc] if self.edge_groups == 1 else list(self.fc)
         k_in = k_edge + 2 * gather_scalars
-        return all(fused.ENABLED and self._fusable(fc, k_in) and fused.supported(table, fc[0].out_features, k_in) for fc in fcs)
+        return all(fused.ENABLED and self._fused_mlp(fc, k_in) and fused.supported(table, fc[0].out_features, k_in)
+                   for fc in fcs)
 
     def _run(self, x, prepared, fcs, from_vec, ew_scalar, n_out, reduce, gather_scalars, scale, shift, residual=None,
              init=None, finalize=True, swap_gathered=False, second_order=True):

@@ -211,7 +211,9 @@ int ddb200_radial_mlp(const float* edge_attr, int64_t ld_ea, int ne, const float
  * per-complex sigma-embedding term of models/cg_model.py:298-301 without materialising edge_attr + sigma per step.
  * w1_images / w2_images / tiles / mtab: the plan built by diffdock_b200/fused.py (operand images [hi | lo | bias] with
  * 16-column-aligned sections, N tiles = whole rows of one path block, dense Clebsch-Gordan tables [path][3][3][5] padded to
- * 48 floats).  Supported shapes: (mul_out, 2l_out+1) in {(48,1),(10,3),(16,1),(4,3),(10,1),(4,1)}, l_in <= 1, at most
+ * 48 floats).  FCBlock = Linear(W1) -> ReLU -> [Linear(Wh_l) -> ReLU for l < n_hidden] -> Linear(W2): wh_images holds the
+ * n_hidden extra H x H layers (tp_weights_layers - 2 of them) as [n_hidden] one-N-tile images of the W2 layout, 128-byte
+ * aligned; n_hidden = 0 with wh_images = NULL is the two-layer FCBlock.  Supported shapes: (mul_out, 2l_out+1) in {(48,1),(10,3),(16,1),(4,3),(10,1),(4,1)}, l_in <= 1, at most
  * 16 paths, spherical harmonics from edge vectors (sh_lmax <= 2), ne + 2 ns <= 144, hidden <= 144.
  * Any base pointer and row stride is accepted.  The rows of a are read with 16-byte loads when ne % 8 == 0, ns % 8 == 0,
  * ld_ea % 4 == 0, edge_attr 16-byte aligned, and (ns > 0) ld_node % 4 == 0 and node 16-byte aligned, and (ea_add given)
@@ -236,6 +238,7 @@ typedef struct ddb200_fused_args {
   int32_t        sh_lmax;
   int64_t        n_edges;     const int32_t* n_edges_dev;      /* capacity (or count if n_edges_dev == NULL)           */
   float*         sum;         int32_t d_out;   float* cnt;     /* [n_dst, d_out] fp32, [n_dst] fp32 or NULL            */
+  const void*    wh_images;   int32_t n_hidden;                /* extra H x H hidden layers (NULL / 0: two-layer FCBlock) */
 } ddb200_fused_args;
 
 int ddb200_fused_conv(const ddb200_fused_args* args, void* stream);
