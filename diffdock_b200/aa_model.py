@@ -1,4 +1,5 @@
-"""Drop-in for the reference's all-atom score model ``models/aa_model.py:AAModel`` (score mode) - SURVEY.md section 8, row f3.
+"""Drop-in for the reference's all-atom model ``models/aa_model.py:AAModel`` (score mode; confidence mode as in
+diffdock_b200/cg_model.py) - SURVEY.md section 8, row f3.
 
 Same constructor keywords, ``forward(data) -> (tr_pred, rot_pred, tor_pred, None)`` contract, ``state_dict`` keys and side
 effects on ``data`` (the cached receptor / atom embeddings of models/aa_model.py:319-333) as the reference class.  It is the
@@ -11,7 +12,7 @@ Two reference behaviours are reproduced on purpose: the reversed groups (residue
 the FORWARD direction's spherical harmonics (:405-406; the coarse-grained model evaluates Y(-v) instead, cg_model.py:556-557),
 and ligand-atom distances go through the ligand distance expansion (:613) into an MLP sized for the cross expansion (:108).
 
-CUDA only, inference only, score mode only.  No CPU fallback.  Like the coarse-grained model the forward has a sync-free
+CUDA only, inference only.  No CPU fallback.  Like the coarse-grained model the forward has a sync-free
 form (``_forward_sync_free``: every per-step neighbour list in a capacity buffer with its live count on the device, the three
 reversed groups as permutations of the forward lists, sigma terms of the four static groups added inside the kernel), so the
 sampler captures the all-atom step in a CUDA graph too; ``_forward_host_sized`` reads the neighbour-list sizes back and is
@@ -55,7 +56,10 @@ class AAModel(CGModel):
                          use_second_order_repr=use_second_order_repr, batch_norm=batch_norm,
                          dynamic_max_cross=dynamic_max_cross, dropout=dropout, smooth_edges=False, odd_parity=odd_parity,
                          separate_noise_schedule=separate_noise_schedule, lm_embedding_type=lm_embedding_type,
-                         confidence_mode=confidence_mode, asyncronous_noise_schedule=asyncronous_noise_schedule,
+                         confidence_mode=confidence_mode, confidence_dropout=confidence_dropout,
+                         confidence_no_batchnorm=confidence_no_batchnorm, num_confidence_outputs=num_confidence_outputs,
+                         atom_num_confidence_outputs=atom_num_confidence_outputs,
+                         asyncronous_noise_schedule=asyncronous_noise_schedule,
                          affinity_prediction=affinity_prediction, parallel=parallel, fixed_center_conv=fixed_center_conv,
                          no_aminoacid_identities=no_aminoacid_identities,
                          include_miscellaneous_atoms=include_miscellaneous_atoms,
@@ -157,7 +161,7 @@ class AAModel(CGModel):
         lig, rec, atom = data['ligand'], data['receptor'], data['atom']
         ns, n_lig = self.ns, lig.batch.shape[0]
         o_r, o_a = n_lig, n_lig + rec.batch.shape[0]
-        tr_sigma, rot_sigma, tor_sigma = self.t_to_sigma(*[data.complex_t[k] for k in ('tr', 'rot', 'tor')])
+        tr_sigma, rot_sigma, tor_sigma = self._sigmas(data)
 
         sig = self.rec_sigma_embedding(self.timestep_emb_func(data.complex_t['tr'])).contiguous()
         rec_node, atom_node = rec.rec_node_attr.clone(), atom.atom_node_attr.clone()
@@ -185,7 +189,7 @@ class AAModel(CGModel):
         """Forward with exactly-sized neighbour lists (the sizes are read back to the host)."""
         lig, rec, atom = data['ligand'], data['receptor'], data['atom']
         ns = self.ns
-        tr_sigma, rot_sigma, tor_sigma = self.t_to_sigma(*[data.complex_t[k] for k in ('tr', 'rot', 'tor')])
+        tr_sigma, rot_sigma, tor_sigma = self._sigmas(data)
         n_lig, n_rec = lig.pos.shape[0], rec.pos.shape[0]
         o_r, o_a = n_lig, n_lig + n_rec
 

@@ -1,6 +1,7 @@
-"""Drop-in for the reference's coarse-grained score model ``models/cg_model.py:CGModel`` (score mode).
+"""Drop-in for the reference's coarse-grained model ``models/cg_model.py:CGModel`` in score and confidence mode.
 
-Same constructor keywords, ``forward(data) -> (tr_pred, rot_pred, tor_pred, sidechain_pred)`` contract, ``state_dict``
+Same constructor keywords, ``forward(data) -> (tr_pred, rot_pred, tor_pred, sidechain_pred)`` contract (confidence mode:
+``(confidence, atom_confidence)``, the times used as sigmas, the head in one ddb200_confidence_head launch), ``state_dict``
 keys and side effects on ``data`` (SURVEY.md section 8(b)); ``utils/sampling.py:116`` can call it unchanged.  What runs
 underneath is H100-native: neighbour search and the tensor-product convolutions (SH + Clebsch-Gordan contraction +
 segmented reduction + BatchNorm/residual epilogue) are hand-written sm_90a kernels behind the C ABI
@@ -20,8 +21,8 @@ from torch import nn
 
 from . import ops
 from .irreps import irreps_str, sh_irreps
-from .layers import (AtomEncoder, GaussianSmearing, _mlp, check_forward, cross_cutoff, cross_graph, edge_cutoff, edge_weight,
-                     ligand_graph, score_heads)
+from .layers import (AtomEncoder, GaussianSmearing, _mlp, check_confidence_widths, check_forward, confidence_head, cross_cutoff,
+                     cross_graph, edge_cutoff, edge_weight, ligand_graph, score_heads)
 from .synthetic import LIG_FEATURE_DIMS as lig_feature_dims, REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims
 from .tensor_layers import TensorProductConvLayer, get_irrep_seq
 from .tp_table import full_tensor_product
@@ -63,13 +64,13 @@ class CGModel(nn.Module):
                  embed_also_ligand=False, atom_confidence=False, sidechain_pred=False, depthwise_convolution=False):
         super().__init__()
         assert parallel == 1, "not implemented"
-        unsupported = dict(confidence_mode=confidence_mode, separate_noise_schedule=separate_noise_schedule,
+        unsupported = dict(separate_noise_schedule=separate_noise_schedule,
                            asyncronous_noise_schedule=asyncronous_noise_schedule,
                            include_miscellaneous_atoms=include_miscellaneous_atoms, sidechain_pred=sidechain_pred,
-                           depthwise_convolution=depthwise_convolution, atom_confidence=atom_confidence)
+                           depthwise_convolution=depthwise_convolution)
         bad = [k for k, v in unsupported.items() if v]
         if bad:
-            raise NotImplementedError(f"{bad}: outside the score-model hot path built so far (SURVEY.md section 8)")
+            raise NotImplementedError(f"{bad}: outside the hot path built so far (SURVEY.md section 8)")
         if lm_embedding_type not in (None, 'precomputed'):
             raise NotImplementedError("on-the-fly ESM embeddings are preprocessing (out of scope); use 'precomputed'")
         self.t_to_sigma, self.device, self.timestep_emb_func = t_to_sigma, device, timestep_emb_func
@@ -83,7 +84,8 @@ class CGModel(nn.Module):
         self.ns, self.nv = ns, nv
         self.scale_by_sigma, self.norm_by_sigma = scale_by_sigma, norm_by_sigma
         self.no_torsion, self.smooth_edges, self.odd_parity = no_torsion, smooth_edges, odd_parity
-        self.confidence_mode = False
+        self.confidence_mode, self.affinity_prediction = confidence_mode, affinity_prediction
+        self.atom_confidence, self.atom_num_confidence_outputs = atom_confidence, atom_num_confidence_outputs
         self.num_conv_layers, self.num_prot_emb_layers = num_conv_layers, num_prot_emb_layers
         self.fixed_center_conv, self.no_aminoacid_identities = fixed_center_conv, no_aminoacid_identities
         self.differentiate_convolutions, self.reduce_pseudoscalars = differentiate_convolutions, reduce_pseudoscalars
@@ -111,6 +113,10 @@ class CGModel(nn.Module):
         if embed_also_ligand:
             self.lig_emb_layers = nn.ModuleList([self.conv(i, 1) for i in range(num_prot_emb_layers)])
         self.conv_layers = self._interaction_stack(4, 2)
+        self._sync_free = None
+        if confidence_mode:
+            self._confidence_heads(confidence_dropout, confidence_no_batchnorm, num_confidence_outputs)
+            return
 
         # translation / rotation head
         self.center_distance_expansion = GaussianSmearing(0.0, center_max_distance, D)
@@ -136,7 +142,25 @@ class CGModel(nn.Module):
         z = np.load(_TABLES)
         self.register_buffer('_so3_table', torch.from_numpy(z['so3_exp_score_norms']).float(), persistent=False)
         self.register_buffer('_torus_table', torch.from_numpy(z['torus_score_norm']).float(), persistent=False)
-        self._sync_free = None
+
+    def _confidence_heads(self, dropout, no_batchnorm, num_confidence_outputs):
+        """``atom_confidence_predictor`` (with atom_confidence) and ``confidence_predictor`` (models/cg_model.py:181-208 =
+        models/aa_model.py:177-211).  The pooled input is the first ns columns of the ligand features and, after three or
+        more convolutions in all (embedding + interaction layers), the last nv (reduce_pseudoscalars) or ns columns."""
+        ns = self.ns
+        self._conf_tail = (self.nv if self.reduce_pseudoscalars else ns) \
+            if self.num_conv_layers + self.num_prot_emb_layers >= 3 else 0
+        n_in = ns + self._conf_tail
+
+        def head(i, o):
+            bn = (lambda: nn.Identity()) if no_batchnorm else (lambda: nn.BatchNorm1d(ns))
+            return nn.Sequential(nn.Linear(i, ns), bn(), nn.ReLU(), nn.Dropout(dropout), nn.Linear(ns, ns), bn(), nn.ReLU(),
+                                 nn.Dropout(dropout), nn.Linear(ns, o))
+        if self.atom_confidence:
+            self.atom_confidence_predictor = head(n_in, self.atom_num_confidence_outputs + ns)
+            n_in = ns
+        self.confidence_predictor = head(n_in, num_confidence_outputs + (1 if self.affinity_prediction else 0))
+        check_confidence_widths(self)
 
     def conv(self, i, groups):
         """Convolution ``i`` of the stack (protein embedding layers first) with ``groups`` radial MLPs."""
@@ -321,7 +345,7 @@ class CGModel(nn.Module):
         a CUDA graph (diffdock_b200/sampling.py)."""
         lig, rec = data['ligand'], data['receptor']
         ns, n_lig = self.ns, lig.batch.shape[0]
-        tr_sigma, rot_sigma, tor_sigma = self.t_to_sigma(*[data.complex_t[k] for k in ('tr', 'rot', 'tor')])
+        tr_sigma, rot_sigma, tor_sigma = self._sigmas(data)
 
         # -- embeddings (models/cg_model.py:272-306) --------------------------------------------------------------
         sig = self.rec_sigma_embedding(self.timestep_emb_func(data.complex_t['tr'])).contiguous()      # [B, ns]
@@ -509,7 +533,7 @@ class CGModel(nn.Module):
         """Forward with exactly-sized neighbour lists (one host read of each edge count): convolution shapes outside the
         fused kernel's templates, or more than 10000 residues per complex."""
         rec, ns = data['receptor'], self.ns
-        tr_sigma, rot_sigma, tor_sigma = self.t_to_sigma(*[data.complex_t[k] for k in ('tr', 'rot', 'tor')])
+        tr_sigma, rot_sigma, tor_sigma = self._sigmas(data)
 
         # -- embeddings (models/cg_model.py:272-306) --------------------------------------------------------------
         sig = self.rec_sigma_embedding(self.timestep_emb_func(data.complex_t['tr']))
@@ -545,5 +569,13 @@ class CGModel(nn.Module):
         node = self._interaction_layers(node, groups, 2, merge=not self.differentiate_convolutions)
         return self._heads(data, c, node[:n_lig], tr_sigma, rot_sigma, tor_sigma, sync_free=False)
 
+    def _sigmas(self, data):
+        """(tr, rot, tor) sigma per complex; the confidence model takes the times as sigmas (models/cg_model.py:312-315)."""
+        t = [data.complex_t[k] for k in ('tr', 'rot', 'tor')]
+        return t if self.confidence_mode else self.t_to_sigma(*t)
+
     def _heads(self, data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_free):
+        """Score mode: ``(tr, rot, tor, None)``; confidence mode: ``(confidence, atom_confidence)``."""
+        if self.confidence_mode:
+            return confidence_head(self, lig_node, c['lig_ptr'])
         return score_heads(self, data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_free) + (None,)

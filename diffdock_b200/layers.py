@@ -77,13 +77,71 @@ def cross_graph(model, data, xpos, x_ptr, r, r_per_graph, expansion, mlp):
     return li, xi, ea, vec, model.get_edge_weight(vec, edge_cutoff(r, r_per_graph, lig.batch, li))
 
 
-def confidence_head(model, data, lig_node):
-    """Mean of the ligand scalars per complex through ``confidence_predictor`` (models/old_cg_model.py:298-299)."""
-    ns, B, batch = model.ns, data.num_graphs, data['ligand'].batch
-    scal = torch.cat([lig_node[:, :ns], lig_node[:, -ns:]], 1) if model.num_conv_layers >= 3 else lig_node[:, :ns]
-    pooled = torch.zeros((B, scal.shape[1]), device=scal.device, dtype=scal.dtype).index_add_(0, batch, scal)
-    pooled = pooled / torch.bincount(batch, minlength=B).clamp(min=1).unsqueeze(1)
-    return model.confidence_predictor(pooled).squeeze(dim=-1)
+def _mlp_dims(seq):
+    """(in, hidden, out) of a confidence MLP: Linear, BN / Identity, ReLU, Dropout, Linear, BN / Identity, ReLU, Dropout,
+    Linear (models/cg_model.py:198-208)."""
+    return seq[0].in_features, seq[0].out_features, seq[8].out_features
+
+
+def check_confidence_widths(model):
+    """Rejects, at construction, confidence heads wider than ddb200_confidence_head takes (DDB200_CONF_MAX_*)."""
+    heads = [model.confidence_predictor] + ([model.atom_confidence_predictor] if getattr(model, 'atom_confidence', False)
+                                            else [])
+    for seq in heads:
+        n_in, h, n_out = _mlp_dims(seq)
+        if seq is not model.confidence_predictor:
+            n_out -= _mlp_dims(model.confidence_predictor)[0]        # the atom outputs; the rest is pooled
+        if n_in > ops.CONF_MAX_IN or h > ops.CONF_MAX_HIDDEN or n_out > ops.CONF_MAX_OUT:
+            raise NotImplementedError(f"confidence head of widths in={n_in} hidden={h} out={n_out}: the confidence kernel "
+                                      f"takes in <= {ops.CONF_MAX_IN}, hidden <= {ops.CONF_MAX_HIDDEN}, "
+                                      f"out <= {ops.CONF_MAX_OUT}")
+
+
+def _pack_mlp(seq):
+    """The packed float32 MLP of ddb200_confidence_head (include/diffdock_b200.h), BatchNorm folded into (scale, shift)."""
+    parts = []
+    for lin, norm in ((seq[0], seq[1]), (seq[4], seq[5]), (seq[8], None)):
+        parts += [lin.weight.detach().float().reshape(-1), lin.bias.detach().float()]
+        if norm is None:
+            continue
+        if isinstance(norm, nn.BatchNorm1d):
+            scale = norm.weight.detach().float() / torch.sqrt(norm.running_var.float() + norm.eps)
+            shift = norm.bias.detach().float() - norm.running_mean.float() * scale
+        else:                                                          # confidence_no_batchnorm: nn.Identity
+            scale, shift = torch.ones_like(lin.bias).float(), torch.zeros_like(lin.bias).float()
+        parts += [scale, shift]
+    return torch.cat(parts).contiguous()
+
+
+def _packed_heads(model):
+    """Packed confidence MLPs of ``model``, rebuilt only when a parameter or buffer changed (load_state_dict, .to())."""
+    seqs = [model.confidence_predictor] + ([model.atom_confidence_predictor] if getattr(model, 'atom_confidence', False)
+                                           else [])
+    key = tuple((t.data_ptr(), t._version) for s in seqs for t in list(s.parameters()) + list(s.buffers()))
+    cache = getattr(model, '_conf_pack', None)
+    if cache is None or cache[0] != key:
+        cache = (key, [_pack_mlp(s) for s in seqs])
+        model._conf_pack = cache
+    return cache[1]
+
+
+def confidence_head(model, lig_node, lig_ptr):
+    """``(confidence [B] or [B, k], atom_confidence [n_lig, k_atom] or zeros [n_lig])`` of the ligand node features in one
+    ddb200_confidence_head launch (models/cg_model.py:354-366, models/old_cg_model.py:296-299): the first ``ns`` columns and
+    the last ``model._conf_tail`` ones, the optional per-atom head, the mean per pose, ``confidence_predictor``."""
+    packs = _packed_heads(model)
+    n_tail = model._conf_tail
+    dims = _mlp_dims(model.confidence_predictor)
+    atom = getattr(model, 'atom_confidence', False)
+    x = lig_node.float()
+    if x.stride(1) != 1:
+        x = x.contiguous()
+    conf, atom_conf = ops.confidence_head(
+        x, lig_ptr, model.ns, n_tail, packs[0], dims, atom_mlp=packs[1] if atom else None,
+        atom_dims=(model.atom_confidence_predictor[0].out_features, model.atom_num_confidence_outputs) if atom else None)
+    if atom_conf is None:
+        atom_conf = torch.zeros((lig_node.shape[0],), device=lig_node.device)
+    return conf.squeeze(dim=-1), atom_conf
 
 
 def _sh_l2(vec):

@@ -21,8 +21,8 @@ from torch import nn
 
 from . import ops
 from .irreps import irreps_str, sh_irreps
-from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_forward, confidence_head, cross_cutoff, cross_graph,
-                     edge_weight, ligand_graph)
+from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_confidence_widths, check_forward, confidence_head,
+                     cross_cutoff, cross_graph, edge_weight, ligand_graph)
 from .synthetic import (LIG_FEATURE_DIMS as lig_feature_dims, REC_ATOM_FEATURE_DIMS as rec_atom_feature_dims,
                         REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims)
 from .tensor_layers import OldTensorProductConvLayer
@@ -87,6 +87,8 @@ class AAOldModel(nn.Module):
         self.confidence_predictor = nn.Sequential(
             nn.Linear(2 * ns if num_conv_layers >= 3 else ns, ns), bn(), nn.ReLU(), nn.Dropout(confidence_dropout),
             nn.Linear(ns, ns), bn(), nn.ReLU(), nn.Dropout(confidence_dropout), nn.Linear(ns, out_dim))
+        self._conf_tail = ns if num_conv_layers >= 3 else 0
+        check_confidence_widths(self)
 
     def load_state_dict(self, state_dict, strict=True, **kw):
         """Reference checkpoints carry e3nn's tensor-product buffers (``*.tp.*``): dropped, the kernels have their own tables."""
@@ -165,4 +167,4 @@ class AAOldModel(nn.Module):
             if l != L - 1:
                 atom = F.pad(atom, (0, at_up.shape[-1] - atom.shape[-1])) + at_up + al_up + ar_up
                 rec = F.pad(rec, (0, rec_up.shape[-1] - rec.shape[-1])) + rec_up + ra_up + rl_up
-        return confidence_head(self, data, lig)
+        return confidence_head(self, lig, ops.segment_ptr(lig_s.batch, B))[0]

@@ -44,8 +44,8 @@ from torch import nn
 from . import ops
 from .cg_model import _TABLES, CGModel, _flat, _i32
 from .irreps import irreps_str, sh_irreps
-from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_forward, confidence_head, cross_cutoff, cross_graph,
-                     edge_weight, ligand_graph, score_heads)
+from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_confidence_widths, check_forward, confidence_head,
+                     cross_cutoff, cross_graph, edge_weight, ligand_graph, score_heads)
 from .synthetic import LIG_FEATURE_DIMS as lig_feature_dims, REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims
 from .tensor_layers import OldTensorProductConvLayer
 from .tp_table import full_tensor_product
@@ -119,6 +119,8 @@ class CGOldModel(nn.Module):
                 nn.Linear(2 * ns if num_conv_layers >= 3 else ns, ns), bn(), nn.ReLU(), nn.Dropout(confidence_dropout),
                 nn.Linear(ns, ns), bn(), nn.ReLU(), nn.Dropout(confidence_dropout),
                 nn.Linear(ns, 2 if affinity_prediction else 1))
+            self._conf_tail = ns if num_conv_layers >= 3 else 0
+            check_confidence_widths(self)
             return
         # score mode: translation / rotation and torsion heads (:156-201)
         S, D = sigma_embed_dim, distance_embed_dim
@@ -159,7 +161,8 @@ class CGOldModel(nn.Module):
     def forward(self, data):                                            # models/old_cg_model.py:203-351
         check_forward(self, data)
         if self.confidence_mode:                                        # times are used as they are (:210)
-            return confidence_head(self, data, self._forward_host_sized(data, data.complex_t['tr']))
+            lig_node = self._forward_host_sized(data, data.complex_t['tr'])
+            return confidence_head(self, lig_node, ops.segment_ptr(data['ligand'].batch, data.num_graphs))[0]
         c = self._static(data)
         tr_sigma, rot_sigma, tor_sigma = self.t_to_sigma(*[data.complex_t[k] for k in ('tr', 'rot', 'tor')])
         sync_free = self.sync_free_capable() and c['rec_max'] <= 10000      # the cross graph's cap (:445) must not bind

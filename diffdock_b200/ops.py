@@ -330,6 +330,34 @@ def crop_select_edges(tgt32, src32, keep, gid32=None, offset=0):
     return out_t[:n], out_s[:n], perm[:n], out_g[:n] if out_g is not None else None, n_dev
 
 
+CONF_MAX_IN, CONF_MAX_HIDDEN, CONF_MAX_OUT = 256, 128, 16       # DDB200_CONF_MAX_* of include/diffdock_b200.h
+
+
+def confidence_head(x, lig_ptr, n_head, n_tail, mlp, dims, atom_mlp=None, atom_dims=None):
+    """ddb200_confidence_head: ``(confidence [B, n_out], atom_confidence [n_lig, n_atom_out] | None)`` from the ligand node
+    features ``x`` [n_lig, D] and the pose pointer ``lig_ptr`` [B+1] (int32, device).  The selected columns are the first
+    ``n_head`` and the last ``n_tail`` of ``x``; ``mlp`` / ``atom_mlp`` are packed MLPs (layout in the header) of
+    ``dims`` = (in, hidden, out) and ``atom_dims`` = (hidden, n_atom_out).  No host synchronisation."""
+    _need_cuda(x, lig_ptr, mlp, atom_mlp)
+    assert x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1
+    assert lig_ptr.dtype == torch.int32 and lig_ptr.is_contiguous()
+    assert mlp.dtype == torch.float32 and mlp.is_contiguous()
+    n_in, n_hidden, n_out = dims
+    B, n_lig, D = lig_ptr.shape[0] - 1, x.shape[0], x.shape[1]
+    conf = torch.empty((B, n_out), dtype=torch.float32, device=x.device)
+    atom_conf, a_h, a_out = None, 0, 0
+    if atom_mlp is not None:
+        assert atom_mlp.dtype == torch.float32 and atom_mlp.is_contiguous()
+        a_h, a_out = atom_dims
+        atom_conf = torch.empty((n_lig, a_out), dtype=torch.float32, device=x.device)
+    rc = _lib.lib().ddb200_confidence_head(_ptr(x), max(x.stride(0), D), D, _ptr(lig_ptr), B, int(n_head), D - int(n_tail),
+                                           int(n_tail), _ptr(atom_mlp), a_h, a_out, _ptr(mlp), n_in, n_hidden, n_out,
+                                           _ptr(conf), _ptr(atom_conf), _stream())
+    _lib.check(rc, 'ddb200_confidence_head')
+    PROFILE.all_launches += 1
+    return conf, atom_conf
+
+
 def csr_sort_by_target(tgt32, n_rows, want_row_ptr=False):
     """Stable device-side sort of an edge list by target: (tgt_sorted int32, perm int64, row_ptr int32 | None);
     ddb200_csr_sort_by_target with a torch-allocated workspace.  No host synchronisation."""

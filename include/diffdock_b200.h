@@ -295,6 +295,31 @@ int ddb200_crop_select_edges(const int32_t* tgt, const int32_t* src, const int32
                              int32_t* out_gid, int32_t* n_selected, void* workspace, size_t* workspace_bytes,
                              void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * ddb200_confidence_head: the confidence head of the confidence models, one CTA per pose b, atoms lig_ptr[b] ..
+ * lig_ptr[b+1] of x [n_lig, n_cols] (row stride ld_x):
+ *   s[a]   = [x[a, 0:n_head] | x[a, tail_off:tail_off + n_tail]]                       (the selected scalar columns)
+ *   with atom_mlp:  y[a] = atom_mlp(s[a]) [n_atom_out + n_in];  atom_confidence[a, 0:n_atom_out] = y[a, 0:n_atom_out];
+ *                   s[a] = y[a, n_atom_out:]
+ *   confidence[b, 0:n_out] = mlp(mean over the pose's atoms of s[a])          (an empty pose: mean = 0)
+ * A packed MLP is Linear -> BN -> ReLU -> Linear -> BN -> ReLU -> Linear in eval mode (Dropout = identity), float32:
+ *   W1 [h, in] row-major | b1 [h] | scale1 [h] | shift1 [h] | W2 [h, h] | b2 | scale2 | shift2 | W3 [out, h] | b3 [out]
+ *   with BatchNorm folded to y = (W x + b) * scale + shift (nn.Identity: scale 1, shift 0).  For atom_mlp: in = n_head +
+ *   n_tail, h = atom_hidden, out = n_atom_out + n_in; for mlp: in = n_in (= n_head + n_tail without atom_mlp), h = n_hidden.
+ * Fixed summation order, no atomics: bit-identical results across calls.  No host synchronisation.
+ * Limits (DDB200_EINVAL beyond them): n_head + n_tail and n_in <= DDB200_CONF_MAX_IN; n_hidden, atom_hidden <=
+ *   DDB200_CONF_MAX_HIDDEN; n_out, n_atom_out <= DDB200_CONF_MAX_OUT.  atom_mlp NULL: no atom head (atom_confidence unused).
+ * Replaces: models/cg_model.py:354-366 / models/aa_model.py:434-455 (scatter_mean + the two nn.Sequential heads) and
+ * models/old_cg_model.py:296-299 / models/old_aa_model.py:283-286.
+ * ------------------------------------------------------------------------------------------------------------- */
+#define DDB200_CONF_MAX_IN 256
+#define DDB200_CONF_MAX_HIDDEN 128
+#define DDB200_CONF_MAX_OUT 16
+int ddb200_confidence_head(const float* x, int64_t ld_x, int64_t n_cols, const int32_t* lig_ptr, int32_t n_poses,
+                           int32_t n_head, int32_t tail_off, int32_t n_tail, const float* atom_mlp, int32_t atom_hidden,
+                           int32_t n_atom_out, const float* mlp, int32_t n_in, int32_t n_hidden, int32_t n_out,
+                           float* confidence, float* atom_confidence, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
