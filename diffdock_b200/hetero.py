@@ -225,10 +225,24 @@ def collate(data_list: List[HeteroGraph]) -> HeteroGraph:
     return out
 
 
+_RECEPTOR_SIDE = ('receptor', 'atom')
+
+
+def _receptor_side(g: HeteroGraph):
+    """(node types, edge types) of the receptor side of a complex: residues, receptor atoms (all-atom graphs) and every
+    edge type touching either."""
+    nts = [k for k in _RECEPTOR_SIDE if k in g._nodes]
+    return nts, [k for k in g._edges if k[0] in nts or k[1] in nts]
+
+
 def _same_receptor(a: HeteroGraph, b: HeteroGraph) -> bool:
-    """Exact equality of everything the model reads from the receptor (cheap identity checks first)."""
-    ra, rb, ea, eb = a['receptor'], b['receptor'], a['receptor', 'receptor'], b['receptor', 'receptor']
-    for sa, sb in ((ra, rb), (ea, eb)):
+    """Exact equality of everything the model reads from the receptor side - residues, and receptor atoms with their edges
+    when the graphs are all-atom ones (cheap identity checks first)."""
+    nts, ets = _receptor_side(a)
+    if (nts, ets) != _receptor_side(b) or 'receptor' not in nts:
+        return False
+    pairs = [(a._nodes[k], b._nodes[k]) for k in nts] + [(a._edges[k], b._edges[k]) for k in ets]
+    for sa, sb in pairs:
         ka = [k for k in sa.keys() if not k.startswith('_')]
         if ka != [k for k in sb.keys() if not k.startswith('_')]:
             return False
@@ -252,53 +266,59 @@ def collate_shared_receptor(data_list: List[HeteroGraph], device, non_blocking=T
     concatenated on the host and uploaded (7.7 MB instead of 246 MB for 32 poses of a 1500-residue complex with 1280-wide
     language-model embeddings); the batch-level tensors are then tiled on the device, so the result is identical to the
     general path, and the receptor store carries ``_unique = (n_nodes_per_copy, n_edges_per_copy, copies)`` so that the
-    score model embeds the receptor once (models/cg_model.py:272-295 recomputes the identical receptor per pose)."""
+    score model embeds the receptor once (models/cg_model.py:272-295 recomputes the identical receptor per pose).
+
+    All-atom graphs (the all-atom models' and the all-atom confidence model's input) get the same treatment for the
+    receptor-atom store and the ('atom', 'atom') / ('atom', 'receptor') edges: one copy uploaded, tiled on the device with
+    per-copy atom and residue offsets, and ``_unique = (n_atoms_per_copy, n_atom_atom_edges_per_copy, copies)`` on the atom
+    store.  An edge type between the receptor side and the ligand takes the general path."""
     B = len(data_list)
     if B < 2 or not all(_same_receptor(data_list[0], d) for d in data_list[1:]):
         return collate(data_list).to(device, non_blocking=non_blocking)
     first = data_list[0]
+    nts, ets = _receptor_side(first)
+    if any(et[0] not in nts or et[1] not in nts for et in ets):
+        return collate(data_list).to(device, non_blocking=non_blocking)
     stripped = []
-    for d in data_list:                       # views without the receptor: ligand / other stores are shared, not copied
+    for d in data_list:                       # views without the receptor side: ligand stores are shared, not copied
         h = HeteroGraph()
         for k, st in d._nodes.items():
-            if k != 'receptor':
+            if k not in nts:
                 h._nodes[k] = st
         for k, st in d._edges.items():
-            if 'receptor' not in k:
+            if k not in ets:
                 h._edges[k] = st
         h._globals.update(d._globals)
         stripped.append(h)
     out = collate(stripped).to(device, non_blocking=non_blocking)
-    rec1, rr1 = first['receptor'], first['receptor', 'receptor']
-    n1 = rec1.num_nodes
-    rec = out['receptor']
-    for k in rec1.keys():
-        if k.startswith('_'):
-            continue
-        v = getattr(rec1, k)
-        if torch.is_tensor(v):
-            dv = v.to(device, non_blocking=non_blocking)
-            setattr(rec, k, dv.repeat((B,) + (1,) * (dv.dim() - 1)) if dv.dim() > 0 else dv)
-        else:
-            setattr(rec, k, [v] * B)
-    rec.batch = torch.arange(B, device=device).repeat_interleave(n1)
-    rec.ptr = torch.arange(B + 1, device=device) * n1
-    rec._unique = (n1, rr1.num_edges, B)
-    rr = out['receptor', 'receptor']
-    for k in rr1.keys():
-        v = getattr(rr1, k)
-        if k == 'edge_index':
-            ei = v.to(device, non_blocking=non_blocking)
-            off = (torch.arange(B, device=device) * n1).repeat_interleave(ei.shape[1])
-            rr.edge_index = ei.repeat(1, B) + off.unsqueeze(0)
-        elif torch.is_tensor(v):
-            dv = v.to(device, non_blocking=non_blocking)
-            setattr(rr, k, dv.repeat((B,) + (1,) * (dv.dim() - 1)))
-        else:
-            setattr(rr, k, [v] * B)
-    for et in first.edge_types:               # other edge types touching the receptor (none on the coarse-grained path)
-        if 'receptor' in et and et != ('receptor', 'receptor'):
-            return collate(data_list).to(device, non_blocking=non_blocking)
+    tile = lambda dv: dv.repeat((B,) + (1,) * (dv.dim() - 1)) if dv.dim() > 0 else dv
+    n1 = {}
+    for nt in nts:
+        st1 = first._nodes[nt]
+        n1[nt] = st1.num_nodes
+        st = out[nt]
+        for k in st1.keys():
+            if k.startswith('_'):
+                continue
+            v = getattr(st1, k)
+            setattr(st, k, tile(v.to(device, non_blocking=non_blocking)) if torch.is_tensor(v) else [v] * B)
+        st.batch = torch.arange(B, device=device).repeat_interleave(n1[nt])
+        st.ptr = torch.arange(B + 1, device=device) * n1[nt]
+        own = first._edges.get((nt, nt))
+        st._unique = (n1[nt], own.num_edges if own is not None else 0, B)
+    for et in ets:
+        st1, st = first._edges[et], out[et]
+        for k in st1.keys():
+            v = getattr(st1, k)
+            if k == 'edge_index':
+                ei = v.to(device, non_blocking=non_blocking)
+                copy_id = torch.arange(B, device=device).repeat_interleave(ei.shape[1])
+                off = torch.stack([copy_id * n1[et[0]], copy_id * n1[et[1]]])
+                st.edge_index = ei.repeat(1, B) + off.to(ei.dtype)
+            elif torch.is_tensor(v):
+                setattr(st, k, tile(v.to(device, non_blocking=non_blocking)))
+            else:
+                setattr(st, k, [v] * B)
     return out
 
 

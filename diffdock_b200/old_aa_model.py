@@ -11,24 +11,72 @@ vectors, OldTensorProductConvLayer on the fully fused wgmma kernel when its shap
 (atom<-ligand, residue<-ligand, residue<-atom) reuse the forward edge attributes AND the forward vector's harmonics, as the
 reference does (:246-266).
 
+Where every convolution has a fused-kernel shape and no complex has more than 10 000 residues or atoms, the forward makes
+no device->host read after the per-batch constants (``_static``, ``_forward_sync_free``), as CGOldModel's score mode does:
+
+1. The residue and atom node embeddings are computed once per batch with the sigma embedding set to zero; each call adds
+   ``M . sigma_emb`` per complex (the encoders are affine in the sigma embedding).  A batch of B poses of one receptor
+   (``_unique`` on the residue and atom stores, diffdock_b200.hetero.collate_shared_receptor) embeds one copy.
+2. The three static edge sets (residue-residue, atom-atom, atom-residue) are CSR-sorted by target once per batch; the
+   residue<-atom group is the atom<-residue list sorted by residue, reading its attributes through ``edge_perm``.  Their
+   edge attributes depend on sigma and are embedded per call (one copy's when the batch holds one receptor at one time).
+3. The ligand graph and the ligand<-residue / ligand<-atom graphs go into capacity buffers with device counts; the
+   atom<-ligand and residue<-ligand groups are permutations of those lists with the forward vector (``vec_sign = +1``).
+4. Nine fused launches per layer, each with its own radial MLP, into one accumulator per (target type, convolution);
+   three chained ddb200_tpconv_finalize calls per target type give ``pad(x) + up + up + up`` in the reference's order.
+5. In a batch of one receptor at one time (``_uniform_t``: the sampler's ranking call at t = 0) the four layer-0 groups that
+   end on residues or atoms and start from them (residue<-residue, residue<-atom, atom<-atom, atom<-residue) see the same
+   inputs in every copy: their messages are computed for copy 0 and added to every copy.
+
 CUDA only, inference only.  No CPU fallback.
 """
 from __future__ import annotations
+
+import os
+import weakref
 
 import torch
 import torch.nn.functional as F
 from torch import nn
 
 from . import ops
+from .cg_model import CGModel, _flat, _i32
 from .irreps import irreps_str, sh_irreps
 from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_confidence_widths, check_forward, confidence_head,
                      cross_cutoff, cross_graph, edge_weight, ligand_graph)
+from .old_cg_model import CGOldModel, sigma_map
 from .synthetic import (LIG_FEATURE_DIMS as lig_feature_dims, REC_ATOM_FEATURE_DIMS as rec_atom_feature_dims,
                         REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims)
 from .tensor_layers import OldTensorProductConvLayer
 
+# target-type rows of each interaction layer: (node type, its three convolutions in the order the reference adds them,
+# models/old_aa_model.py:280-285); convolution k of layer l is conv_layers[9 l + k]
+_LIG_SUM, _REC_SUM, _ATOM_SUM = (0, 2, 1), (6, 8, 7), (3, 4, 5)
+
+
+def _uniq(st, B, n_edges):
+    """True when ``st`` carries ``_unique = (nodes, edges, copies)`` for this batch of B copies."""
+    u = getattr(st, '_unique', None)
+    return u is not None and u[2] == B and u[0] * B == st.pos.shape[0] and u[1] * B == n_edges
+
+
+def _csr(tgt, n_rows):
+    """(target int32 sorted stably, order int64) of an edge list."""
+    if tgt.shape[0] == 0:
+        return _i32(tgt), torch.zeros(0, dtype=torch.long, device=tgt.device)
+    t32, order, _ = ops.csr_sort_by_target(_i32(tgt), n_rows)
+    return t32, order
+
 
 class AAOldModel(nn.Module):
+    # the ligand graph, the cross graphs and the per-batch constants of the sync-free path are the score models'
+    _static_sync_free = CGModel._static_sync_free
+    _ligand_edges_sync_free = CGModel._ligand_edges_sync_free
+    _cross_graph_sync_free = CGModel._cross_graph_sync_free
+    _cross_edge_embedding = CGModel._cross_edge_embedding
+    _edge_embed_in_kernel = CGModel._edge_embed_in_kernel
+    _bn = staticmethod(CGOldModel._bn)
+
     def __init__(self, t_to_sigma, device, timestep_emb_func, in_lig_edge_features=4, sigma_embed_dim=32, sh_lmax=2,
                  ns=16, nv=4, num_conv_layers=2, lig_max_radius=5, rec_max_radius=30, cross_max_distance=250,
                  center_max_distance=30, distance_embed_dim=32, cross_distance_embed_dim=32, no_torsion=False,
@@ -89,6 +137,7 @@ class AAOldModel(nn.Module):
             nn.Linear(ns, ns), bn(), nn.ReLU(), nn.Dropout(confidence_dropout), nn.Linear(ns, out_dim))
         self._conf_tail = ns if num_conv_layers >= 3 else 0
         check_confidence_widths(self)
+        self._sync_free = None
 
     def load_state_dict(self, state_dict, strict=True, **kw):
         """Reference checkpoints carry e3nn's tensor-product buffers (``*.tp.*``): dropped, the kernels have their own tables."""
@@ -111,6 +160,188 @@ class AAOldModel(nn.Module):
     @torch.no_grad()
     def forward(self, data):                                            # models/old_aa_model.py:202-286
         check_forward(self, data)
+        if self.sync_free_capable():
+            c = self._static(data)
+            if max(c['rec_max'], c['atom_max']) <= 10000:      # the cross graphs' cap (:454, :470) must not bind
+                return confidence_head(self, self._forward_sync_free(data, c), c['lig_ptr'])[0]
+        return self._forward_host_sized(data)
+
+    def sync_free_capable(self):
+        """The forward runs without a device->host read after the per-batch constants when every one of the 9 L
+        convolutions has a shape the fully fused kernel supports."""
+        if self._sync_free is None:
+            ok = os.environ.get('DDB200_SYNC_FREE', '1') != '0'
+            self._sync_free = bool(ok and all(layer.fused_capable(self.ns, self.ns) for layer in self.conv_layers))
+        return self._sync_free
+
+    # ---------------------------------------------------------------------------------------------------------
+    def _static(self, data):
+        """Per-batch constants, cached on ``data`` (host reads of the node counts): the sigma-free residue and atom node
+        embeddings with their sigma maps, the static edge sets CSR-sorted by target in the joint numbering
+        [ligand | residues | atoms] with the complex of each edge, copy 0 of them in the local numbering
+        [residues | atoms] of one copy when the batch holds ``copies`` identical receptors, and the ligand / cross-graph
+        constants of CGModel._static_sync_free."""
+        rec, atom, lig = data['receptor'], data['atom'], data['ligand']
+        rr, aa, ar, ll = data['receptor', 'receptor'], data['atom', 'atom'], data['atom', 'receptor'], data['ligand', 'ligand']
+        hit = getattr(rr, '_b200_v10aa', None)
+        if hit is not None and hit[0]() is self:
+            return hit[1]
+        B, S = data.num_graphs, self.sigma_embed_dim
+        n_lig, n_rec, n_atom = lig.batch.shape[0], rec.pos.shape[0], atom.pos.shape[0]
+        o_r, o_a = n_lig, n_lig + n_rec
+        N = o_a + n_atom
+        rr_ei, aa_ei, ar_ei = rr.edge_index.long(), aa.edge_index.long(), ar.edge_index.long()
+        copies = B if B > 1 and _uniq(rec, B, rr_ei.shape[1]) and _uniq(atom, B, aa_ei.shape[1]) \
+            and ar_ei.shape[1] % B == 0 else 1
+        n1r, n1a = n_rec // copies, n_atom // copies
+        c = {'copies': copies, 'n1': (n1r, n1a)}
+        # node embeddings with the sigma embedding set to zero (:401, :424), one copy, the LM layer included
+        for key, st, enc, n1 in (('rec', rec, self.rec_node_embedding, n1r), ('atom', atom, self.atom_node_embedding, n1a)):
+            x1 = st.x[:n1].float()
+            base = enc(torch.cat([x1, x1.new_zeros((n1, S))], 1))
+            c[key + '_base'] = base.repeat(copies, 1) if copies > 1 else base
+            c[key + '_sigma_map'] = sigma_map(enc, S, st.x.shape[1])
+        c['rec_gid'], c['atom_gid'] = rec.batch, atom.batch
+        # static edge sets (:404-445, :486): row 0 = convolution target, vector gathered - target, sigma of the target's complex
+        rp, ap = rec.pos.float(), atom.pos.float()
+        spec = {'rr': (rr_ei[0] + o_r, rr_ei[1] + o_r, rp[rr_ei[1]] - rp[rr_ei[0]], rec.batch[rr_ei[0]], self.rec_max_radius),
+                'aa': (aa_ei[0] + o_a, aa_ei[1] + o_a, ap[aa_ei[1]] - ap[aa_ei[0]], atom.batch[aa_ei[0]], self.lig_max_radius),
+                'ar': (ar_ei[0] + o_a, ar_ei[1] + o_r, rp[ar_ei[1]] - ap[ar_ei[0]], atom.batch[ar_ei[0]], None)}
+        for k, (tgt, src, vec, gid, max_r) in spec.items():
+            t32, order = _csr(tgt, N)
+            vec = vec[order].contiguous()
+            c[k] = dict(tgt=t32, src=_i32(src[order]), vec=vec, gid=_i32(gid[order]),
+                        ew=_flat(self.get_edge_weight(vec, max_r)) if max_r is not None else None)
+        # residue <- atom (:264-266): the atom <- residue edges sorted by residue, forward attributes and vector
+        t32, order = _csr(c['ar']['src'].long(), N)
+        c['ra'] = dict(tgt=t32, src=c['ar']['tgt'][order].contiguous(), perm=_i32(order))
+        if copies > 1:
+            # copy 0 of every sorted list comes first (its targets sort first); the other copies read its attributes
+            local = {'rr': (o_r, 0, o_r, 0), 'aa': (o_a, n1r, o_a, n1r), 'ar': (o_a, n1r, o_r, 0)}
+            for k, (to, tb, so, sb) in local.items():
+                d, E = c[k], c[k]['tgt'].shape[0]
+                e1 = E // copies
+                d['perm'] = _i32(torch.arange(E, device=rp.device) % max(e1, 1))
+                c[k + '0'] = dict(tgt=_i32(d['tgt'][:e1] - to + tb), src=_i32(d['src'][:e1] - so + sb),
+                                  vec=d['vec'][:e1].contiguous(), row=torch.zeros(e1, dtype=torch.int32, device=rp.device),
+                                  ew=d['ew'][:e1].contiguous() if d['ew'] is not None else None)
+            e1 = c['ra']['tgt'].shape[0] // copies
+            c['ra']['perm_shared'] = _i32(c['ra']['perm'] % max(e1, 1))
+            c['ra0'] = dict(tgt=_i32(c['ra']['tgt'][:e1] - o_r), src=_i32(c['ra']['src'][:e1] - o_a + n1r),
+                            perm=c['ra']['perm'][:e1].contiguous())
+        # ligand graph and cross-graph constants (CGModel._static_sync_free) and the atom side of the ligand<-atom graph
+        c['rec_ptr'], c['atom_ptr'], c['lig_ptr'] = (ops.segment_ptr(s.batch, B) for s in (rec, atom, lig))
+        c['rr_tgt_batch'] = rec.batch[rr_ei[0]]
+        bonds = ll.edge_index[:, lig.edge_mask].long()
+        c['bonds'], c['n_bonds'] = bonds, int(bonds.shape[1])
+        c['bond_batch'] = lig.batch[bonds[0]] if bonds.shape[1] else None
+        self._static_sync_free(data, c)
+        atom_cnt, lig_cnt = c['atom_ptr'][1:] - c['atom_ptr'][:-1], c['lig_ptr'][1:] - c['lig_ptr'][:-1]
+        c['atom_max'] = int(atom_cnt.max()) if B else 0
+        c['cap_la'] = int((lig_cnt.long() * atom_cnt.long()).sum())      # every ligand atom x every atom of its complex
+        c['atom_batch32'] = _i32(atom.batch)
+        rr._b200_v10aa = (weakref.ref(self), c)
+        return c
+
+    def _static_edge_attr(self, sig, vec, row, mlp, gs):
+        """``mlp(cat[sigma_emb of the edge's complex, gs(|vec|)])`` (:409-410, :431-432, :489) with ``sig`` [rows, S] and
+        ``row`` the sigma row of each edge; an empty edge set (e.g. a receptor without contact edges) has none."""
+        if vec.shape[0] == 0:
+            return vec.new_zeros((0, self.ns))
+        return self._cross_edge_embedding(sig, vec, row, None, mlp, gs)
+
+    def _forward_sync_free(self, data, c):
+        """Ligand node features after the interaction layers without a device->host read (module docstring, 1-5)."""
+        lig, rec, atom = data['ligand'], data['receptor'], data['atom']
+        ns, n_lig = self.ns, lig.batch.shape[0]
+        o_r, o_a = n_lig, n_lig + rec.pos.shape[0]
+        N = o_a + atom.pos.shape[0]
+        shared = c['copies'] > 1 and getattr(data, '_uniform_t', False)     # one receptor at one time
+        tr_sigma = data.complex_t['tr']                                      # confidence mode: the times are the sigmas
+        sig = self.timestep_emb_func(tr_sigma)                               # [B, S], per complex
+
+        # -- residue / atom embeddings and the static groups (:400-445, :486-491) ----------------------------------------
+        rec_node = c['rec_base'] + (sig @ c['rec_sigma_map'].t())[c['rec_gid']]
+        atom_node = c['atom_base'] + (sig @ c['atom_sigma_map'].t())[c['atom_gid']]
+        emb = {'rr': (self.rec_edge_embedding, self.rec_distance_expansion),
+               'aa': (self.atom_edge_embedding, self.lig_distance_expansion),
+               'ar': (self.ar_edge_embedding, self.rec_distance_expansion)}
+        g, g0 = {}, {}
+        for k, (mlp, gs) in emb.items():
+            d = c[k]
+            if shared:      # one copy's attributes; the copies read them through edge_perm
+                d0 = c[k + '0']
+                ea = self._static_edge_attr(sig[:1], d0['vec'], d0['row'], mlp, gs)
+                g[k] = (d['tgt'], d['src'], ea, d0['vec'], d0['ew'], dict(edge_perm=d['perm']))
+                g0[k] = (d0['tgt'], d0['src'], ea, d0['vec'], d0['ew'], {})
+            else:
+                ea = self._static_edge_attr(sig, d['vec'], d['gid'], mlp, gs)
+                g[k] = (d['tgt'], d['src'], ea, d['vec'], d['ew'], {})
+        ra = c['ra']
+        g['ra'] = (ra['tgt'], ra['src'], g['ar'][2], g['ar'][3], None,
+                   dict(edge_perm=ra['perm_shared'] if shared else ra['perm']))
+        if shared:
+            g0['ra'] = (c['ra0']['tgt'], c['ra0']['src'], g0['ar'][2], g0['ar'][3], None, dict(edge_perm=c['ra0']['perm']))
+
+        # -- ligand graph (:358-398) and ligand cross graphs (:447-485) --------------------------------------------------
+        g_ll = self._ligand_edges_sync_free(data, c)
+        lig_node = self.lig_node_embedding(torch.cat([lig.x.float(), lig.node_sigma_emb], 1))
+        r, rpg = cross_cutoff(self, tr_sigma)
+        # atom <- ligand and residue <- ligand reuse the forward attributes and harmonics (:254, :262): vec_sign = +1
+        g_lr, g_rl = self._cross_graph_sync_free(data, c, rec.pos.float().contiguous(), c['rec_ptr'], c['rec_batch32'],
+                                                 c['rec_max'], c['cap_cross'], r, rpg, o_r, self.lr_edge_embedding,
+                                                 self.cross_distance_expansion, vec_sign=1.0)
+        g_la, g_al = self._cross_graph_sync_free(data, c, atom.pos.float().contiguous(), c['atom_ptr'], c['atom_batch32'],
+                                                 c['atom_max'], c['cap_la'], float(self.lig_max_radius), None, o_a,
+                                                 self.la_edge_embedding, self.cross_distance_expansion, vec_sign=1.0)
+        groups = {0: (g_ll, n_lig), 1: (g_lr, n_lig), 2: (g_la, n_lig), 3: (g['aa'], N), 4: (g_al, N), 5: (g['ar'], N),
+                  6: (g['rr'], o_a), 7: (g_rl, o_a), 8: (g['ra'], o_a)}
+
+        # -- interaction layers (:229-286) --------------------------------------------------------------------------------
+        x = torch.cat([lig_node, rec_node, atom_node], 0)
+        L, C = self.num_conv_layers, self.conv_layers
+        for l in range(L):
+            last = l == L - 1
+            convs = C[9 * l:9 * l + 9]
+            ks = (0, 1, 2) if last else range(9)
+            acc = self._shared_static_messages(x, c, g0, o_r, o_a, N, convs) if (l == 0 and shared and not last) else {}
+            for k in ks:        # raw sums per convolution; rows of a sum: its target type's rows in the joint numbering
+                if k not in acc:
+                    acc[k] = convs[k].accumulate_group(x, groups[k][0], 0, groups[k][1], ns)
+            rows = [(0, n_lig, _LIG_SUM)] + ([] if last else [(o_r, o_a, _REC_SUM), (o_a, N, _ATOM_SUM)])
+            out = torch.empty((n_lig if last else N, convs[0].out_size), device=x.device)
+            for lo, hi, order in rows:      # pad(x) + up_a + up_b + up_c (:280-285)
+                part = x[lo:hi]
+                for j, k in enumerate(order):
+                    s, n = acc[k]
+                    part = ops.tpconv_finalize(s[lo:hi], n[lo:hi], True, *self._bn(convs[k]), residual=part,
+                                               out=out[lo:hi] if j == 2 else None)
+            x = out
+        return x
+
+    def _shared_static_messages(self, x, c, g0, o_r, o_a, N, convs):
+        """Layer-0 sums of the four groups between residues and atoms (residue<-residue, residue<-atom, atom<-atom,
+        atom<-residue) for a batch of B poses of ONE receptor at ONE time: their node features and edge attributes are the
+        same in every copy, so the sums are computed for copy 0 (local numbering [residues | atoms] of one copy) and
+        added to every copy's rows."""
+        B, (n1r, n1a) = c['copies'], c['n1']
+        x0 = torch.cat([x[o_r:o_r + n1r], x[o_a:o_a + n1a]], 0)
+        D = convs[0].out_size
+        acc = {}
+        for k, key, lo, n_full in ((6, 'rr', o_r, o_a), (8, 'ra', o_r, o_a), (3, 'aa', o_a, N), (5, 'ar', o_a, N)):
+            to_atom = lo == o_a
+            n_loc, m = (n1r + n1a, n1a) if to_atom else (n1r, n1r)
+            s0, n0 = convs[k].accumulate_group(x0, g0[key], 0, n_loc, self.ns)
+            s = torch.zeros((n_full, D), device=x.device)
+            n = torch.zeros((n_full,), device=x.device)
+            s[lo:].view(B, m, D).add_(s0[n_loc - m:].unsqueeze(0))
+            n[lo:].view(B, m).add_(n0[n_loc - m:].unsqueeze(0))
+            acc[k] = (s, n)
+        return acc
+
+    def _forward_host_sized(self, data):
+        """Exactly-sized neighbour lists (one host read of each edge count), every convolution through
+        OldTensorProductConvLayer.forward: layer shapes outside the fused kernel, or more than 10 000 residues / atoms."""
         lig_s, rec_s, atom_s = data['ligand'], data['receptor'], data['atom']
         B, ns, L, C = data.num_graphs, self.ns, self.num_conv_layers, self.conv_layers
         tr_sigma = data.complex_t['tr']                                 # confidence mode: times are used as they are (:209)

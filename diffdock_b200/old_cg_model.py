@@ -30,11 +30,15 @@ shape, else ``_forward_host_sized``.  What the v1.0 wiring changes on that path 
 4. rec<-lig uses Y(rec - lig) unnegated (:265): the reverse permutation of the cross list with ``vec_sign = +1``.
 5. Layer-0 rec<-rec messages of a one-receptor, one-time batch are computed for one copy and added to all copies.
 
+Confidence mode runs the same sync-free forward with the times as sigmas, then the one-kernel confidence head; where its
+conditions fail it keeps the host-sized forward.
+
 CUDA only, inference only.  No CPU fallback.
 """
 from __future__ import annotations
 
 import os
+import weakref
 
 import numpy as np
 import torch
@@ -49,6 +53,26 @@ from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_confidence_wi
 from .synthetic import LIG_FEATURE_DIMS as lig_feature_dims, REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims
 from .tensor_layers import OldTensorProductConvLayer
 from .tp_table import full_tensor_product
+
+
+def sigma_map(enc, S, x_cols):
+    """``M`` [ns, S] with enc(cat[x, s]) = enc(cat[x, 0]) + M s for the OldAtomEncoder ``enc`` and its input
+    ``cat[x (x_cols columns), sigma embedding (S columns)]``: the encoder reads its scalar columns and (with an LM embedding)
+    the last ``lm_embedding_dim`` columns of that input (models/layers.py:103-116); the sigma columns can fall in either."""
+    nc, nsf = enc.num_categorical_features, enc.num_scalar_features
+    cols = torch.arange(x_cols, x_cols + S)                              # where the sigma embedding sits
+    W = enc.linear.weight.detach()
+    m = W.new_zeros((W.shape[0], S))
+    j = cols - nc
+    ok = (j >= 0) & (j < nsf)
+    m[:, ok] = W[:, j[ok]]
+    if enc.lm_embedding_type is not None:
+        W_lm, lm = enc.lm_embedding_layer.weight.detach(), enc.lm_embedding_dim
+        m = W_lm[:, :W.shape[0]] @ m
+        j = cols - (x_cols + S - lm)
+        ok = j >= 0
+        m[:, ok] += W_lm[:, W.shape[0] + j[ok]]
+    return m.contiguous()
 
 
 class CGOldModel(nn.Module):
@@ -113,6 +137,7 @@ class CGOldModel(nn.Module):
             r2l.append(OldTensorProductConvLayer(**p))
         self.lig_conv_layers, self.rec_conv_layers = nn.ModuleList(lig), nn.ModuleList(rec)
         self.lig_to_rec_conv_layers, self.rec_to_lig_conv_layers = nn.ModuleList(l2r), nn.ModuleList(r2l)
+        self._sync_free = None
         if confidence_mode:
             bn = (lambda: nn.Identity()) if confidence_no_batchnorm else (lambda: nn.BatchNorm1d(ns))
             self.confidence_predictor = nn.Sequential(
@@ -146,7 +171,6 @@ class CGOldModel(nn.Module):
         z = np.load(_TABLES)        # score-norm tables (utils/so3.py:59, utils/torus.py:72-76), not in the state_dict
         self.register_buffer('_so3_table', torch.from_numpy(z['so3_exp_score_norms']).float(), persistent=False)
         self.register_buffer('_torus_table', torch.from_numpy(z['torus_score_norm']).float(), persistent=False)
-        self._sync_free = None
 
     def load_state_dict(self, state_dict, strict=True, **kw):
         """Reference checkpoints carry e3nn's tensor-product buffers (``*.tp.*``, and ``final_tp_tor.*`` in score mode):
@@ -161,6 +185,10 @@ class CGOldModel(nn.Module):
     def forward(self, data):                                            # models/old_cg_model.py:203-351
         check_forward(self, data)
         if self.confidence_mode:                                        # times are used as they are (:210)
+            if self.sync_free_capable():
+                c = self._static(data)
+                if c['rec_max'] <= 10000:
+                    return confidence_head(self, self._forward_sync_free(data, c, data.complex_t['tr']), c['lig_ptr'])[0]
             lig_node = self._forward_host_sized(data, data.complex_t['tr'])
             return confidence_head(self, lig_node, ops.segment_ptr(data['ligand'].batch, data.num_graphs))[0]
         c = self._static(data)
@@ -170,8 +198,8 @@ class CGOldModel(nn.Module):
         return score_heads(self, data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_free)
 
     def sync_free_capable(self):
-        """Score mode: the forward runs without any host synchronisation (and so inside a CUDA graph) when every
-        convolution of the stack has a shape the fully fused kernel supports."""
+        """The forward runs without any host synchronisation after the per-batch constants (and so, in score mode, inside
+        a CUDA graph) when every convolution of the stack has a shape the fully fused kernel supports."""
         if self._sync_free is None:
             ok = os.environ.get('DDB200_SYNC_FREE', '1') != '0'
             for convs in (self.lig_conv_layers, self.rec_conv_layers, self.lig_to_rec_conv_layers, self.rec_to_lig_conv_layers):
@@ -189,8 +217,9 @@ class CGOldModel(nn.Module):
         """Per-batch constants of the score model, cached on ``data`` (one host read per batch): the sigma-free part of the
         receptor node embedding, the contact graph in CSR order by target, and those of CGModel._static_sync_free."""
         rec, rr, lig, ll = data['receptor'], data['receptor', 'receptor'], data['ligand'], data['ligand', 'ligand']
-        if hasattr(rr, '_b200_v10'):
-            return rr._b200_v10
+        hit = getattr(rr, '_b200_v10', None)
+        if hit is not None and hit[0]() is self:      # per model: the score and confidence models may share the batch
+            return hit[1]
         B, n_lig, ns = data.num_graphs, lig.batch.shape[0], self.ns
         ei = rr.edge_index.long()
         uniq = getattr(rec, '_unique', None)       # (nodes, edges, copies): the batch holds `copies` identical receptors
@@ -203,7 +232,7 @@ class CGOldModel(nn.Module):
         x1 = rec.x[:n1].float()
         base = self.rec_node_embedding(torch.cat([x1, x1.new_zeros((n1, self.sigma_embed_dim))], 1))
         c['rec_base'] = base.repeat(copies, 1) if copies > 1 else base
-        c['rec_sigma_map'] = self._rec_sigma_map(rec.x.shape[1])
+        c['rec_sigma_map'] = sigma_map(self.rec_node_embedding, self.sigma_embed_dim, rec.x.shape[1])
         c['rec_gid'] = rec.batch                # complex of each residue: the sigma terms are per complex, not per batch
         # contact graph in CSR order by target (edge_index[0]); vector gathered - target (:406)
         tgt, order = torch.sort(ei[0], stable=True)
@@ -226,28 +255,8 @@ class CGOldModel(nn.Module):
         c['bonds'], c['n_bonds'] = bonds, int(bonds.shape[1])
         c['bond_batch'] = lig.batch[bonds[0]] if bonds.shape[1] else None
         self._static_sync_free(data, c)
-        rr._b200_v10 = c
+        rr._b200_v10 = (weakref.ref(self), c)
         return c
-
-    def _rec_sigma_map(self, x_cols):
-        """``M`` [ns, S] with rec_node_embedding(cat[x, s]) = rec_node_embedding(cat[x, 0]) + M s for the encoder input
-        ``cat[x (x_cols columns), sigma embedding]``: the encoder reads its scalar columns and (with an LM embedding) the
-        last ``lm_embedding_dim`` columns of that input (models/layers.py:103-116); the sigma columns can fall in either."""
-        enc, S = self.rec_node_embedding, self.sigma_embed_dim
-        nc, nsf = enc.num_categorical_features, enc.num_scalar_features
-        cols = torch.arange(x_cols, x_cols + S)                              # where the sigma embedding sits
-        W = enc.linear.weight.detach()
-        m = W.new_zeros((W.shape[0], S))
-        j = cols - nc
-        ok = (j >= 0) & (j < nsf)
-        m[:, ok] = W[:, j[ok]]
-        if enc.lm_embedding_type is not None:
-            W_lm, lm = enc.lm_embedding_layer.weight.detach(), enc.lm_embedding_dim
-            m = W_lm[:, :W.shape[0]] @ m
-            j = cols - (x_cols + S - lm)
-            ok = j >= 0
-            m[:, ok] += W_lm[:, W.shape[0] + j[ok]]
-        return m.contiguous()
 
     def _forward_sync_free(self, data, c, tr_sigma):
         """Ligand node features after the interaction layers without a device->host read: capacity buffers with device

@@ -18,7 +18,7 @@ import torch
 
 from . import ops
 from .diffusion_utils import set_time
-from .hetero import collate, collate_shared_receptor
+from .hetero import HeteroGraph, collate, collate_shared_receptor
 
 
 def randomize_position(data_list, no_torsion, no_random, tr_sigma_max, pocket_knowledge=False, pocket_cutoff=7,
@@ -472,12 +472,21 @@ def sampling(data_list, model, inference_steps, tr_schedule, rot_schedule, tor_s
             data_list[b0 + i]['ligand'].pos = g['ligand'].pos[i * n:n * (i + 1)]
         if confidence_model is not None:
             if conf_batches is not None:
-                cg = collate(copy.deepcopy(conf_batches[batch_id]))
-                cg['ligand'].pos = g['ligand'].pos.cpu()
-                cg = cg.to(device)
-                if getattr(confidence_model_args, 'crop_beyond', None) is not None:     # utils/sampling.py:213-217
-                    cg = crop_receptor(cg, confidence_model_args.crop_beyond)
+                crop = getattr(confidence_model_args, 'crop_beyond', None)
+                items = conf_batches[batch_id]
+                if isinstance(items[0], HeteroGraph) and not (crop is not None and confidence_model_args.all_atoms):
+                    # one receptor copy uploaded and tiled on the device; the collate builds new stores, so the caller's
+                    # items are never written to, and the final positions stay on the device
+                    cg = collate_shared_receptor(items, device)
+                    cg['ligand'].pos = g['ligand'].pos.clone()
+                else:
+                    cg = collate(copy.deepcopy(items))
+                    cg['ligand'].pos = g['ligand'].pos.cpu()
+                    cg = cg.to(device)
+                if crop is not None:                                                    # utils/sampling.py:213-217
+                    cg = crop_receptor(cg, crop)
                 set_time(cg, 0, 0, 0, 0, b, confidence_model_args.all_atoms, device)
+                cg._uniform_t = True                 # every graph of the batch is ranked at t = 0
                 out = confidence_model(cg)
             else:
                 out = confidence_model(g)
