@@ -26,6 +26,8 @@ SIGNATURES = {
                                   _vp]),
     'ddb200_pose_update_dev': (_int, [_vp, _i64, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint64,
                                       _vp, _int, _vp, _vp]),
+    'ddb200_pose_update_packed': (_int, [_vp, _i64, _vp, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint64,
+                                         _vp, _int, _vp, _vp, _vp]),
     'ddb200_philox_probe': (_int, [C.c_uint64, _i64, C.c_uint32, C.c_uint32, _int, _vp, _vp, _vp]),
     'ddb200_graph_fill': (_int, [_vp, _vp, _vp, _vp, _vp, C.c_float, _i64, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                  _vp, _vp, _int, _vp, _int, _int, _vp]),

@@ -21,6 +21,7 @@ from torch import nn
 
 from . import ops
 from .irreps import irreps_str, sh_irreps
+from .hetero import receptor_blocks
 from .layers import (AtomEncoder, GaussianSmearing, _mlp, check_confidence_widths, check_forward, confidence_head, cross_cutoff,
                      cross_graph, edge_cutoff, edge_weight, ligand_graph, score_heads)
 from .synthetic import LIG_FEATURE_DIMS as lig_feature_dims, REC_RESIDUE_FEATURE_DIMS as rec_residue_feature_dims
@@ -47,6 +48,36 @@ def _rr_joint(c, n_lig):
     if n_lig not in c.setdefault('rr_tgt32', {}):
         c['rr_tgt32'][n_lig] = (_i32(c['rr_tgt'] + n_lig), _i32(c['rr_src'] + n_lig))
     return c['rr_tgt32'][n_lig]
+
+
+def receptor_tiles(rec, B, ei):
+    """Index maps between a batch whose receptor store carries a block layout (``hetero.receptor_blocks``) and its distinct
+    receptors, numbered by concatenating copy 0 of each one's first block; None without a layout.  ``nodes`` / ``edges``:
+    batch rows of those copies; ``edge_index``: their contact edges in the distinct numbering; ``node_map`` [n_rec] /
+    ``edge_map`` [E]: the distinct row of every batch node / edge; ``sorted_rows`` / ``sorted_shift``: the rows of the copies
+    in the contact graph sorted stably by target (targets of a copy sort together, copies in batch order) and what turns
+    their batch node numbers into distinct ones."""
+    blocks = receptor_blocks(rec, B, ei.shape[1])
+    if blocks is None:
+        return None
+    dev = ei.device
+    ar = lambda a, b: torch.arange(a, b, device=dev)
+    first, nodes, edges, shift, uoff, ueoff = {}, [], [], [], {}, {}
+    n_u = e_u = 0
+    for noff, eoff, n1, e1, cp, uid in blocks:
+        if uid in first:
+            continue
+        first[uid] = True
+        uoff[uid], ueoff[uid] = n_u, e_u
+        nodes.append(ar(noff, noff + n1))
+        edges.append(ar(eoff, eoff + e1))
+        shift.append(torch.full((e1,), noff - n_u, dtype=torch.long, device=dev))
+        n_u, e_u = n_u + n1, e_u + e1
+    nodes, edges, shift = torch.cat(nodes), torch.cat(edges), torch.cat(shift)
+    node_map = torch.cat([(uoff[uid] + ar(0, n1)).repeat(cp) for _, _, n1, _, cp, uid in blocks])
+    edge_map = torch.cat([(ueoff[uid] + ar(0, e1)).repeat(cp) for _, _, _, e1, cp, uid in blocks])
+    return dict(nodes=nodes, edges=edges, edge_index=ei[:, edges] - shift, node_map=node_map, edge_map=edge_map,
+                sorted_rows=edges, sorted_shift=shift)
 
 
 class CGModel(nn.Module):
@@ -218,26 +249,28 @@ class CGModel(nn.Module):
         B = data.num_graphs
         c = {}
         ei = rr.edge_index.long()
-        uniq = getattr(rec, '_unique', None)       # (nodes, edges, copies): the batch holds `copies` identical receptors
-        if uniq is not None and uniq[2] == B and uniq[0] * B == rec.pos.shape[0] and uniq[1] * B == ei.shape[1]:
-            # N poses of one complex (inference.py:236-239): embed the receptor ONCE and tile the result; the reference
-            # recomputes the identical 1280-wide embedding for every pose of the batch (models/cg_model.py:272-295)
-            copies, n1, e1 = B, uniq[0], uniq[1]
+        # copies of the same receptor (N poses of one complex, inference.py:236-239, or several ligands against one protein
+        # in a packed batch): embed each distinct receptor ONCE and tile the result; the reference recomputes the identical
+        # 1280-wide embedding for every pose of the batch (models/cg_model.py:272-295)
+        tiles = receptor_tiles(rec, B, ei)
+        c['tiles'] = tiles
+        if tiles is None:
+            x1, pos1, ei1 = rec.x, rec.pos, ei
         else:
-            copies, n1, e1 = 1, rec.pos.shape[0], ei.shape[1]
-        ei1 = ei[:, :e1]
-        vec = (rec.pos[ei1[1]] - rec.pos[ei1[0]]).float()
+            x1, pos1, ei1 = rec.x[tiles['nodes']], rec.pos[tiles['nodes']], tiles['edge_index']
+        vec = (pos1[ei1[1]] - pos1[ei1[0]]).float()
         rec_edge_attr = self.rec_edge_embedding(self.rec_distance_expansion(vec.norm(dim=-1)))
-        rec_node_attr = self.rec_node_embedding(rec.x[:n1])
+        rec_node_attr = self.rec_node_embedding(x1)
         if self.rec_emb_layers:     # input of the embedding layers: a cropped step runs them over its own contact graph
-            c['rec_node_pre'] = rec_node_attr.repeat(copies, 1)
+            c['rec_node_pre'] = rec_node_attr[tiles['node_map']] if tiles is not None else rec_node_attr
         ew = self.get_edge_weight(vec, self.rec_max_radius)
         for layer in self.rec_emb_layers:
             ea_ = torch.cat([rec_edge_attr, rec_node_attr[ei1[0], :self.ns], rec_node_attr[ei1[1], :self.ns]], -1)
             rec_node_attr = layer(rec_node_attr, ei1, ea_, None, edge_weight=ew, edge_vec=vec)
-        if copies > 1:
-            vec, rec_edge_attr, rec_node_attr = vec.repeat(B, 1), rec_edge_attr.repeat(B, 1), rec_node_attr.repeat(B, 1)
-            ew = ew.repeat(B, 1) if torch.is_tensor(ew) else ew
+        if tiles is not None:
+            em = tiles['edge_map']
+            vec, rec_edge_attr, rec_node_attr = vec[em], rec_edge_attr[em], rec_node_attr[tiles['node_map']]
+            ew = ew[em] if torch.is_tensor(ew) else ew
         rec.rec_node_attr, rr.rec_edge_attr, rr.edge_weight = rec_node_attr, rec_edge_attr, ew
         rr.edge_sh = None   # evaluated inside the convolution kernel from the edge vectors; kept for attribute parity
         # CSR order of the static receptor graph (target = edge_index[0])
@@ -487,30 +520,33 @@ class CGModel(nn.Module):
                 (b_tgt, b_src, ea, vec, ew, dict(n_edges_dev=n_dev, edge_perm=perm, vec_sign=vec_sign)))
 
     def _shared_receptor_messages(self, data, c, rec, rec_node, sig, n_lig):
-        """Layer-0 receptor<-receptor messages when the batch holds B poses of ONE complex at ONE diffusion time: the residue
-        features entering the first interaction layer (static embedding + sigma embedding) and the contact graph are then the
-        same in every copy, so the messages are computed for one copy (E/B edges) and added to all copies' accumulators.
-        The reference recomputes them per pose (models/cg_model.py:342-349 over the B-fold receptor).  Needs the sampler's
+        """Layer-0 receptor<-receptor messages when the batch holds copies of the same receptors (``c['tiles']``) at ONE
+        diffusion time: the residue features entering the first interaction layer (static embedding + sigma embedding) and
+        the contact graph are then the same in every copy of a receptor, so the messages are computed once per distinct
+        receptor - one accumulation over the concatenated copy-0 graphs - and added to all copies' accumulators.  The
+        reference recomputes them per pose (models/cg_model.py:342-349 over the B-fold receptor).  Needs the sampler's
         promise that all graphs of the batch share t (``data._uniform_t``; the model API allows per-graph times)."""
-        uniq = getattr(rec, '_unique', None)
-        if uniq is None or not getattr(data, '_uniform_t', False) or not self.differentiate_convolutions:
+        tiles = c['tiles']
+        if tiles is None or not getattr(data, '_uniform_t', False) or not self.differentiate_convolutions:
             return None
-        n1, e1, B = uniq
-        if B < 2 or n1 * B != rec_node.shape[0] or c['rr_tgt'].shape[0] != e1 * B:
-            return None
+        n_u = tiles['nodes'].shape[0]
+        if n_u == rec_node.shape[0]:
+            return None                        # no receptor repeats: nothing to share
         layer = self.conv_layers[0]
-        if 'rr0' not in c:          # copy 0 of the CSR-sorted contact graph (targets of copy 0 sort first), local numbering
-            c['rr0'] = (_i32(c['rr_tgt'][:e1]), _i32(c['rr_src'][:e1]), c['rr_ea'][:e1].contiguous(),
-                        c['rr_vec'][:e1].contiguous(), _flat(c['rr_ew'][:e1]) if c['rr_ew'] is not None else None)
+        if 'rr0' not in c:          # copy 0 of each distinct receptor's CSR-sorted contact graph, numbered as tiles['nodes']
+            rows = tiles['sorted_rows']
+            c['rr0'] = (_i32(c['rr_tgt'][rows] - tiles['sorted_shift']), _i32(c['rr_src'][rows] - tiles['sorted_shift']),
+                        c['rr_ea'][rows].contiguous(), c['rr_vec'][rows].contiguous(),
+                        _flat(c['rr_ew'][rows]) if c['rr_ew'] is not None else None)
         t0, s0, ea0, vec0, ew0 = c['rr0']
-        zero_idx = c.setdefault('rr0_zero', torch.zeros(e1, dtype=torch.int32, device=ea0.device))
+        zero_idx = c.setdefault('rr0_zero', torch.zeros(t0.shape[0], dtype=torch.int32, device=ea0.device))
         g0 = (t0, s0, ea0, vec0, ew0, dict(ea_add=sig[:1].contiguous(), ea_add_idx=zero_idx))
-        sum0, cnt0 = layer.accumulate_group(rec_node[:n1], g0, 2, n1, gather_scalars=self.ns)
+        sum0, cnt0 = layer.accumulate_group(rec_node[tiles['nodes']], g0, 2, n_u, gather_scalars=self.ns)
         N = n_lig + rec_node.shape[0]
         sum_buf = torch.zeros((N, layer.out_size), dtype=torch.float32, device=sum0.device)
         cnt_buf = torch.zeros((N,), dtype=torch.float32, device=sum0.device)
-        sum_buf[n_lig:].view(B, n1, layer.out_size).add_(sum0.unsqueeze(0))
-        cnt_buf[n_lig:].view(B, n1).add_(cnt0.unsqueeze(0))
+        sum_buf[n_lig:].add_(sum0[tiles['node_map']])
+        cnt_buf[n_lig:].add_(cnt0[tiles['node_map']])
         return sum_buf, cnt_buf
 
     def _edge_embed_in_kernel(self, mlp, gs):

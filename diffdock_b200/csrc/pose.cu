@@ -3,7 +3,8 @@
 // utils/geometry.py:246-276 batched Kabsch - a Python loop over rotatable bonds with host-sync asserts and a cuSOLVER
 // batched SVD in the reference).
 //
-// Per pose b (all poses of a batch are copies of one ligand, as in the reference's sampler):
+// Per pose b (all poses of a batch are copies of one ligand, as in the reference's sampler, or - packed - each pose with its
+// own ligand layout):
 //   perturb = a * score + c * z                       (a, c: host scalars of the SDE step, one pair per dof type)
 //   rigid   = R(rot) (pos - centroid) + tr + centroid (axis-angle -> quaternion -> matrix, pytorch3d formulas)
 //   flex    = rigid, then for every rotatable bond r in order: atoms of mask[r] rotate about pos[u]-pos[v] through
@@ -31,8 +32,10 @@ __device__ __forceinline__ void axis_angle_to_matrix(float ax, float ay, float a
   M[6] = two_s * (i * k - j * r);     M[7] = two_s * (j * k + i * r);     M[8] = 1 - two_s * (i * i + j * j);
 }
 
-__device__ void block_sum(double* vals, int n, double* red, int tid, int nthreads) {
-  // vals: per-thread partials (n of them); result broadcast in red[0..n)
+__device__ __forceinline__ void block_sum(double* vals, int n, double* red, int tid, int nthreads) {
+  // vals: per-thread partials (n of them); result broadcast in red[0..n).  Inlined with a constant n, so that vals stays in
+  // registers.
+#pragma unroll
   for (int q = 0; q < n; ++q) {
     double v = vals[q];
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -45,33 +48,47 @@ __device__ void block_sum(double* vals, int n, double* red, int tid, int nthread
     red[32 * n + tid] = v;
   }
   __syncthreads();
+#pragma unroll
   for (int q = 0; q < n; ++q) vals[q] = red[32 * n + q];
   __syncthreads();
 }
 
-// Jacobi eigen-decomposition of a symmetric 3x3 (fp64): A = V diag(w) V^T
-__device__ void jacobi3(double A[3][3], double V[3][3], double w[3]) {
+__device__ __forceinline__ void swap3(double a[3], double b[3]) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) { const double t = a[c]; a[c] = b[c]; b[c] = t; }
+}
+
+// Jacobi eigen-decomposition of a symmetric 3x3 (fp64): A = V diag(w) V^T.  Every index is a compile-time constant after
+// unrolling, so A and V stay in registers.
+__device__ __forceinline__ void jacobi3(double A[3][3], double V[3][3], double w[3]) {
+#pragma unroll
   for (int i = 0; i < 3; ++i)
+#pragma unroll
     for (int j = 0; j < 3; ++j) V[i][j] = (i == j);
   for (int sweep = 0; sweep < 30; ++sweep) {
     const double off = fabs(A[0][1]) + fabs(A[0][2]) + fabs(A[1][2]);
     if (off < 1e-300 || off < 1e-18 * (fabs(A[0][0]) + fabs(A[1][1]) + fabs(A[2][2]))) break;
+#pragma unroll
     for (int p = 0; p < 2; ++p)
+#pragma unroll
       for (int q = p + 1; q < 3; ++q) {
         if (fabs(A[p][q]) < 1e-300) continue;
         const double theta = (A[q][q] - A[p][p]) / (2.0 * A[p][q]);
         const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
         const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+#pragma unroll
         for (int k = 0; k < 3; ++k) {
           const double akp = A[k][p], akq = A[k][q];
           A[k][p] = c * akp - s * akq;
           A[k][q] = s * akp + c * akq;
         }
+#pragma unroll
         for (int k = 0; k < 3; ++k) {
           const double apk = A[p][k], aqk = A[q][k];
           A[p][k] = c * apk - s * aqk;
           A[q][k] = s * apk + c * aqk;
         }
+#pragma unroll
         for (int k = 0; k < 3; ++k) {
           const double vkp = V[k][p], vkq = V[k][q];
           V[k][p] = c * vkp - s * vkq;
@@ -118,14 +135,30 @@ struct PoseNoise {
   int philox;
 };
 
-__global__ void pose_update_kernel(const float* pos, int n_atoms, int n_bonds,
-                                   const int* __restrict__ bond_u, const int* __restrict__ bond_v,
+// Where pose b lives.  Uniform batch (layout == NULL): every pose is a copy of one ligand of n_atoms atoms and n_bonds
+// rotatable bonds, pose-major.  Packed batch: row b of layout [n_poses, 6] int32 = (atom_off, n_atoms, bond_off, n_bonds,
+// tor_off, mask_off): rows of pos / out, rows of bond_u / bond_v (local atom numbering), first entry in tor_score / tor_z,
+// first byte of the pose's [n_bonds, n_atoms] mask block.  A packed pose with n_atoms outside [1, max_atoms] (the size the
+// shared memory was sized for) or a negative bond count is left untouched and sets *err = 1.
+__global__ void pose_update_kernel(const float* pos, int n_atoms, int n_bonds, const int* __restrict__ layout, int max_atoms,
+                                   int* err, const int* __restrict__ bond_u, const int* __restrict__ bond_v,
                                    const unsigned char* __restrict__ mask, const float* __restrict__ tr_score,
                                    const float* __restrict__ rot_score, const float* __restrict__ tor_score,
                                    const float* __restrict__ tr_z, const float* __restrict__ rot_z,
                                    const float* __restrict__ tor_z, float a_tr, float c_tr, float a_rot, float c_rot,
                                    float a_tor, float c_tor, int use_torsion, const PoseNoise nz, float* out) {
   extern __shared__ float sm[];
+  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  size_t atom_off = (size_t)b * n_atoms, tor_off = (size_t)b * n_bonds;
+  if (layout) {
+    const int* d = layout + 6 * (size_t)b;
+    atom_off = (size_t)d[0]; n_atoms = d[1]; n_bonds = d[3]; tor_off = (size_t)d[4];
+    if (n_atoms < 1 || n_atoms > max_atoms || n_bonds < 0) {     // uniform over the CTA: nothing below runs
+      if (tid == 0) *err = 1;
+      return;
+    }
+    bond_u += d[2]; bond_v += d[2]; mask += d[5];
+  }
   const int step = nz.step_dev ? *nz.step_dev : 0;
   if (nz.coef_dev) {         // SDE coefficients of this step from a device table: the host never touches the step loop
     const float* cf = nz.coef_dev + 6 * (long long)step;
@@ -135,8 +168,7 @@ __global__ void pose_update_kernel(const float* pos, int n_atoms, int n_bonds,
   float* flex = rig + 3 * n_atoms;         // [n_atoms*3]
   float* mat = flex + 3 * n_atoms;         // [16]
   double* red = reinterpret_cast<double*>(mat + 16);   // [32*9 + 16]
-  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
-  const float* p = pos + (size_t)b * n_atoms * 3;
+  const float* p = pos + atom_off * 3;
 
   // centroid
   double part[9];
@@ -168,7 +200,7 @@ __global__ void pose_update_kernel(const float* pos, int n_atoms, int n_bonds,
     flex[3 * i] = nx; flex[3 * i + 1] = ny; flex[3 * i + 2] = nz;
   }
   __syncthreads();
-  float* o = out + (size_t)b * n_atoms * 3;
+  float* o = out + atom_off * 3;
   if (!use_torsion || n_bonds == 0) {
     for (int i = tid; i < 3 * n_atoms; i += nt) o[i] = rig[i];
     return;
@@ -181,13 +213,14 @@ __global__ void pose_update_kernel(const float* pos, int n_atoms, int n_bonds,
     if (tid == 0) {
       float ax = flex[3 * u] - pvx, ay = flex[3 * u + 1] - pvy, az = flex[3 * u + 2] - pvz;
       const float nrm = sqrtf(ax * ax + ay * ay + az * az);
-      float zq = tor_z ? tor_z[(size_t)b * n_bonds + r] : 0.f;
+      float zq = tor_z ? tor_z[tor_off + r] : 0.f;
       if (nz.philox) {
         float z4[4];
         philox_normal4(nz.seed, nz.pose_key[b], (uint32_t)step, 2u + (uint32_t)(r >> 2), z4);
-        zq = z4[r & 3];
+        const int j = r & 3;                 // selected by value: a run-time index would put z4 on the stack
+        zq = j == 0 ? z4[0] : j == 1 ? z4[1] : j == 2 ? z4[2] : z4[3];
       }
-      const float ang = a_tor * tor_score[(size_t)b * n_bonds + r] + c_tor * zq;
+      const float ang = a_tor * tor_score[tor_off + r] + c_tor * zq;
       ax = ax / nrm * ang; ay = ay / nrm * ang; az = az / nrm * ang;
       axis_angle_to_matrix(ax, ay, az, mat);
     }
@@ -229,11 +262,12 @@ __global__ void pose_update_kernel(const float* pos, int n_atoms, int n_bonds,
     for (int r = 0; r < 3; ++r)
       for (int c = 0; c < 3; ++c) K[r][c] = H[r][0] * H[c][0] + H[r][1] * H[c][1] + H[r][2] * H[c][2];
     jacobi3(K, V, w);
-    int i0 = 0, i1 = 1, i2 = 2;   // sort eigenvalues descending
-    if (w[i0] < w[i1]) { int t = i0; i0 = i1; i1 = t; }
-    if (w[i0] < w[i2]) { int t = i0; i0 = i2; i2 = t; }
-    if (w[i1] < w[i2]) { int t = i1; i1 = i2; i2 = t; }
-    double u1[3] = {V[0][i0], V[1][i0], V[2][i0]}, u2[3] = {V[0][i1], V[1][i1], V[2][i1]};
+    // sort eigenvalues descending, moving the eigenvectors by value (no indexing by a run-time index: registers only)
+    double u1[3] = {V[0][0], V[1][0], V[2][0]}, u2[3] = {V[0][1], V[1][1], V[2][1]}, u3s[3] = {V[0][2], V[1][2], V[2][2]};
+    double w0 = w[0], w1 = w[1], w2 = w[2];
+    if (w0 < w1) { const double t = w0; w0 = w1; w1 = t; swap3(u1, u2); }
+    if (w0 < w2) { const double t = w0; w0 = w2; w2 = t; swap3(u1, u3s); }
+    if (w1 < w2) { const double t = w1; w1 = w2; w2 = t; swap3(u2, u3s); }
     double v1[3], v2[3];
     for (int c = 0; c < 3; ++c) {
       v1[c] = H[0][c] * u1[0] + H[1][c] * u1[1] + H[2][c] * u1[2];
@@ -248,8 +282,10 @@ __global__ void pose_update_kernel(const float* pos, int n_atoms, int n_bonds,
     double n2 = sqrt(v2[0] * v2[0] + v2[1] * v2[1] + v2[2] * v2[2]);
     if (!(n2 > 1e-10 * n1)) {        // complete the frame with the coordinate axis least aligned with v1
       int k = fabs(v1[0]) <= fabs(v1[1]) ? 0 : 1;
-      if (fabs(v1[2]) < fabs(v1[k])) k = 2;
-      for (int c = 0; c < 3; ++c) v2[c] = (c == k) - v1[k] * v1[c];
+      double v1k = k == 0 ? v1[0] : v1[1];
+      if (fabs(v1[2]) < fabs(v1k)) { k = 2; v1k = v1[2]; }
+#pragma unroll
+      for (int c = 0; c < 3; ++c) v2[c] = (c == k) - v1k * v1[c];
       n2 = sqrt(v2[0] * v2[0] + v2[1] * v2[1] + v2[2] * v2[2]);
     }
     for (int c = 0; c < 3; ++c) v2[c] /= n2;
@@ -272,6 +308,34 @@ __global__ void pose_update_kernel(const float* pos, int n_atoms, int n_bonds,
   }
 }
 
+// Shared-memory size for ligands of up to max_atoms atoms, the opt-in above 48 KB, the launch.
+int launch_pose_update(const float* pos, int64_t n_poses, int n_atoms, int n_bonds, const int32_t* layout, int max_atoms,
+                       int32_t* err, const int32_t* bond_u, const int32_t* bond_v, const uint8_t* mask_rotate,
+                       const float* tr_score, const float* rot_score, const float* tor_score, const float* tr_z,
+                       const float* rot_z, const float* tor_z, const float* coef6, int use_torsion, const PoseNoise& nz,
+                       float* out_pos, void* stream) {
+  if (n_poses == 0) return 0;
+  const size_t smem = sizeof(float) * (6 * (size_t)max_atoms + 16) + sizeof(double) * (32 * 9 + 16) + 16;
+  if (smem > 200 * 1024) return DDB200_ESMEM;
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(pose_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+  }
+  const float c0 = coef6 ? coef6[0] : 0.f, c1 = coef6 ? coef6[1] : 0.f, c2 = coef6 ? coef6[2] : 0.f;
+  const float c3 = coef6 ? coef6[3] : 0.f, c4 = coef6 ? coef6[4] : 0.f, c5 = coef6 ? coef6[5] : 0.f;
+  pose_update_kernel<<<(unsigned)n_poses, 128, smem, (cudaStream_t)stream>>>(
+      pos, n_atoms, n_bonds, layout, max_atoms, err, bond_u, bond_v, mask_rotate, tr_score, rot_score, tor_score, tr_z,
+      rot_z, tor_z, c0, c1, c2, c3, c4, c5, use_torsion, nz, out_pos);
+  return (int)cudaGetLastError();
+}
+
+PoseNoise device_noise(const float* coef_table, const int32_t* step_dev, uint64_t seed, const int64_t* pose_key) {
+  PoseNoise nz;
+  nz.coef_dev = coef_table; nz.step_dev = step_dev; nz.seed = seed;
+  nz.pose_key = reinterpret_cast<const long long*>(pose_key); nz.philox = pose_key != nullptr;
+  return nz;
+}
+
 }  // namespace
 
 extern "C" int ddb200_pose_update(const float* pos, int64_t n_poses, int n_atoms, int n_bonds, const int32_t* bond_u,
@@ -282,17 +346,9 @@ extern "C" int ddb200_pose_update(const float* pos, int64_t n_poses, int n_atoms
   if (!pos || !out_pos || !tr_score || !rot_score || !coef6 || n_poses < 0 || n_atoms <= 0 || n_bonds < 0)
     return DDB200_EINVAL;
   if (use_torsion && n_bonds > 0 && (!bond_u || !bond_v || !mask_rotate || !tor_score)) return DDB200_EINVAL;
-  if (n_poses == 0) return 0;
-  const size_t smem = sizeof(float) * (6 * (size_t)n_atoms + 16) + sizeof(double) * (32 * 9 + 16) + 16;
-  if (smem > 200 * 1024) return DDB200_ESMEM;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(pose_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-  }
-  pose_update_kernel<<<(unsigned)n_poses, 128, smem, (cudaStream_t)stream>>>(
-      pos, n_atoms, n_bonds, bond_u, bond_v, mask_rotate, tr_score, rot_score, tor_score, tr_z, rot_z, tor_z, coef6[0],
-      coef6[1], coef6[2], coef6[3], coef6[4], coef6[5], use_torsion, PoseNoise{}, out_pos);
-  return (int)cudaGetLastError();
+  return launch_pose_update(pos, n_poses, n_atoms, n_bonds, nullptr, n_atoms, nullptr, bond_u, bond_v, mask_rotate,
+                            tr_score, rot_score, tor_score, tr_z, rot_z, tor_z, coef6, use_torsion, PoseNoise{}, out_pos,
+                            stream);
 }
 
 // Same update with the step's SDE coefficients read from DEVICE memory (row *step_dev of coef_table [n_steps, 6]; step_dev
@@ -309,20 +365,26 @@ extern "C" int ddb200_pose_update_dev(const float* pos, int64_t n_poses, int n_a
   if (!pos || !out_pos || !tr_score || !rot_score || !coef_table || n_poses < 0 || n_atoms <= 0 || n_bonds < 0)
     return DDB200_EINVAL;
   if (use_torsion && n_bonds > 0 && (!bond_u || !bond_v || !mask_rotate || !tor_score)) return DDB200_EINVAL;
-  if (n_poses == 0) return 0;
-  const size_t smem = sizeof(float) * (6 * (size_t)n_atoms + 16) + sizeof(double) * (32 * 9 + 16) + 16;
-  if (smem > 200 * 1024) return DDB200_ESMEM;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(pose_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-  }
-  PoseNoise nz;
-  nz.coef_dev = coef_table; nz.step_dev = step_dev; nz.seed = seed;
-  nz.pose_key = reinterpret_cast<const long long*>(pose_key); nz.philox = pose_key != nullptr;
-  pose_update_kernel<<<(unsigned)n_poses, 128, smem, (cudaStream_t)stream>>>(
-      pos, n_atoms, n_bonds, bond_u, bond_v, mask_rotate, tr_score, rot_score, tor_score, tr_z, rot_z, tor_z, 0.f, 0.f, 0.f,
-      0.f, 0.f, 0.f, use_torsion, nz, out_pos);
-  return (int)cudaGetLastError();
+  return launch_pose_update(pos, n_poses, n_atoms, n_bonds, nullptr, n_atoms, nullptr, bond_u, bond_v, mask_rotate,
+                            tr_score, rot_score, tor_score, tr_z, rot_z, tor_z, nullptr, use_torsion,
+                            device_noise(coef_table, step_dev, seed, pose_key), out_pos, stream);
+}
+
+// ddb200_pose_update_dev over poses of different ligands: pose b reads its layout from row b of the device descriptor
+// (see pose_update_kernel).  The host never reads the descriptor; max_atoms sizes the shared memory.
+extern "C" int ddb200_pose_update_packed(const float* pos, int64_t n_poses, const int32_t* layout, int max_atoms,
+                                         const int32_t* bond_u, const int32_t* bond_v, const uint8_t* mask_rotate,
+                                         const float* tr_score, const float* rot_score, const float* tor_score,
+                                         const float* tr_z, const float* rot_z, const float* tor_z,
+                                         const float* coef_table, const int32_t* step_dev, uint64_t seed,
+                                         const int64_t* pose_key, int use_torsion, int32_t* err, float* out_pos,
+                                         void* stream) {
+  if (!pos || !out_pos || !tr_score || !rot_score || !coef_table || !layout || !err || n_poses < 0 || max_atoms <= 0)
+    return DDB200_EINVAL;
+  if (use_torsion && (!bond_u || !bond_v || !mask_rotate || !tor_score)) return DDB200_EINVAL;
+  return launch_pose_update(pos, n_poses, 0, 0, layout, max_atoms, err, bond_u, bond_v, mask_rotate, tr_score, rot_score,
+                            tor_score, tr_z, rot_z, tor_z, nullptr, use_torsion,
+                            device_noise(coef_table, step_dev, seed, pose_key), out_pos, stream);
 }
 
 // Diagnostics / tests: out[4 * i .. 4 * i + 3] = the four normals of Philox block (seed, pose_key, step, block0 + i).

@@ -11,6 +11,7 @@ from __future__ import annotations
 import copy
 from typing import Dict, List
 
+import numpy as np
 import torch
 
 
@@ -273,14 +274,43 @@ def collate_shared_receptor(data_list: List[HeteroGraph], device, non_blocking=T
     per-copy atom and residue offsets, and ``_unique = (n_atoms_per_copy, n_atom_atom_edges_per_copy, copies)`` on the atom
     store.  An edge type between the receptor side and the ligand takes the general path."""
     B = len(data_list)
-    if B < 2 or not all(_same_receptor(data_list[0], d) for d in data_list[1:]):
+    if B < 2:
         return collate(data_list).to(device, non_blocking=non_blocking)
-    first = data_list[0]
+    out = _collate_receptor_blocks([data_list], device, non_blocking)
+    if out is None:
+        return collate(data_list).to(device, non_blocking=non_blocking)
+    for nt in _receptor_side(data_list[0])[0]:
+        n1, e1, _, _ = out[nt]._blocks[0]
+        out[nt]._unique = (n1, e1, B)
+        del out[nt].__dict__['_blocks']
+    return out
+
+
+def _collate_receptor_blocks(complexes, device, non_blocking=True):
+    """``collate(concatenated pose lists).to(device)`` with each DISTINCT receptor uploaded once and tiled on the device, or
+    None when some complex's poses do not share one receptor (or an edge type joins the receptor side to the ligand).
+    Consecutive complexes with the same receptor form one block; every receptor-side node store gets ``_blocks`` = one
+    ``(nodes per copy, own edges per copy, copies, distinct receptor id)`` per block, in batch order."""
+    items = [d for poses in complexes for d in poses]
+    first = items[0]
     nts, ets = _receptor_side(first)
     if any(et[0] not in nts or et[1] not in nts for et in ets):
-        return collate(data_list).to(device, non_blocking=non_blocking)
+        return None
+    if not all(_same_receptor(poses[0], d) for poses in complexes for d in poses[1:]):
+        return None
+    reps, blocks = [], []              # distinct receptors (one pose each); [distinct id, copies] per block
+    for poses in complexes:
+        if blocks and _same_receptor(reps[blocks[-1][0]], poses[0]):
+            blocks[-1][1] += len(poses)
+            continue
+        uid = next((u for u, r in enumerate(reps) if _same_receptor(r, poses[0])), None)
+        if uid is None:
+            uid = len(reps)
+            reps.append(poses[0])
+        blocks.append([uid, len(poses)])
+    B = len(items)
     stripped = []
-    for d in data_list:                       # views without the receptor side: ligand stores are shared, not copied
+    for d in items:                           # views without the receptor side: ligand stores are shared, not copied
         h = HeteroGraph()
         for k, st in d._nodes.items():
             if k not in nts:
@@ -291,34 +321,132 @@ def collate_shared_receptor(data_list: List[HeteroGraph], device, non_blocking=T
         h._globals.update(d._globals)
         stripped.append(h)
     out = collate(stripped).to(device, non_blocking=non_blocking)
-    tile = lambda dv: dv.repeat((B,) + (1,) * (dv.dim() - 1)) if dv.dim() > 0 else dv
-    n1 = {}
+    up = {}                                   # (distinct id, store key, attribute) -> device tensor, uploaded once
+
+    def dev(u, key, k, v):
+        if (u, key, k) not in up:
+            up[(u, key, k)] = v.to(device, non_blocking=non_blocking)
+        return up[(u, key, k)]
+    tile = lambda dv, c: dv.repeat((c,) + (1,) * (dv.dim() - 1)) if dv.dim() > 0 else dv
+    n1 = {nt: [r._nodes[nt].num_nodes for r in reps] for nt in nts}
     for nt in nts:
-        st1 = first._nodes[nt]
-        n1[nt] = st1.num_nodes
         st = out[nt]
-        for k in st1.keys():
+        for k in first._nodes[nt].keys():
             if k.startswith('_'):
                 continue
-            v = getattr(st1, k)
-            setattr(st, k, tile(v.to(device, non_blocking=non_blocking)) if torch.is_tensor(v) else [v] * B)
-        st.batch = torch.arange(B, device=device).repeat_interleave(n1[nt])
-        st.ptr = torch.arange(B + 1, device=device) * n1[nt]
-        own = first._edges.get((nt, nt))
-        st._unique = (n1[nt], own.num_edges if own is not None else 0, B)
-    for et in ets:
-        st1, st = first._edges[et], out[et]
-        for k in st1.keys():
-            v = getattr(st1, k)
-            if k == 'edge_index':
-                ei = v.to(device, non_blocking=non_blocking)
-                copy_id = torch.arange(B, device=device).repeat_interleave(ei.shape[1])
-                off = torch.stack([copy_id * n1[et[0]], copy_id * n1[et[1]]])
-                st.edge_index = ei.repeat(1, B) + off.to(ei.dtype)
-            elif torch.is_tensor(v):
-                setattr(st, k, tile(v.to(device, non_blocking=non_blocking)))
+            vals = [getattr(r._nodes[nt], k) for r in reps]
+            if torch.is_tensor(vals[0]):
+                setattr(st, k, torch.cat([tile(dev(u, nt, k, vals[u]), c) for u, c in blocks]))
             else:
-                setattr(st, k, [v] * B)
+                setattr(st, k, [vals[u] for u, c in blocks for _ in range(c)])
+        per_copy = torch.tensor([n1[nt][u] for u, c in blocks for _ in range(c)], device=device)
+        st.batch = torch.arange(B, device=device).repeat_interleave(per_copy)
+        st.ptr = torch.cat([torch.zeros(1, dtype=per_copy.dtype, device=device), torch.cumsum(per_copy, 0)])
+        own = [r._edges.get((nt, nt)) for r in reps]
+        st._blocks = tuple((n1[nt][u], own[u].num_edges if own[u] is not None else 0, c, u) for u, c in blocks)
+    for et in ets:
+        st = out[et]
+        for k in first._edges[et].keys():
+            vals = [getattr(r._edges[et], k) for r in reps]
+            if k == 'edge_index':
+                parts, off0, off1 = [], 0, 0
+                for u, c in blocks:
+                    ei = dev(u, et, k, vals[u])
+                    copy_id = torch.arange(c, device=device).repeat_interleave(ei.shape[1])
+                    off = torch.stack([off0 + copy_id * n1[et[0]][u], off1 + copy_id * n1[et[1]][u]])
+                    parts.append(ei.repeat(1, c) + off.to(ei.dtype))
+                    off0, off1 = off0 + c * n1[et[0]][u], off1 + c * n1[et[1]][u]
+                st.edge_index = torch.cat(parts, 1)
+            elif torch.is_tensor(vals[0]):
+                setattr(st, k, torch.cat([tile(dev(u, et, k, vals[u]), c) for u, c in blocks]))
+            else:
+                setattr(st, k, [vals[u] for u, c in blocks for _ in range(c)])
+    return out
+
+
+def receptor_blocks(st, num_graphs, n_edges):
+    """The receptor block layout of a batch, ``[(node offset, edge offset, nodes per copy, edges per copy, copies, distinct
+    id)]``, from ``_blocks`` (collate_packed) or ``_unique`` (collate_shared_receptor) when it describes this batch - every
+    graph in exactly one copy, nodes and edges summing to the store's - else None."""
+    blocks = getattr(st, '_blocks', None)
+    if blocks is None:
+        u = getattr(st, '_unique', None)
+        blocks = None if u is None else ((u[0], u[1], u[2], 0),)
+    if blocks is None:
+        return None
+    out, noff, eoff = [], 0, 0
+    for n1, e1, c, uid in blocks:
+        out.append((noff, eoff, n1, e1, c, uid))
+        noff, eoff = noff + n1 * c, eoff + e1 * c
+    if sum(b[4] for b in out) != num_graphs or noff != st.num_nodes or eoff != n_edges:
+        return None
+    return out
+
+
+def pose_layout(complexes):
+    """The per-pose descriptor of ddb200_pose_update_packed for the concatenated pose lists, on the host: ``(layout [n_poses,
+    6] int32, bond_u int32, bond_v int32, mask uint8 (flat), max_atoms)``.  Rotatable bonds and masks are read from each
+    complex's first pose, as ``sampling`` does; every pose must have the same atom and rotatable-bond counts."""
+    rows, bu, bv, masks = [], [], [], []
+    atom_off = tor_off = bond_off = mask_off = 0
+    max_atoms = 0
+    for poses in complexes:
+        lig0 = poses[0]['ligand']
+        n = int(lig0.num_nodes)
+        ei = poses[0]['ligand', 'ligand'].edge_index
+        rot = ei.T[lig0.edge_mask.cpu()] if ei.numel() else ei.T.reshape(0, 2)
+        nb = int(rot.shape[0])
+        mask = np.asarray(lig0.mask_rotate[0] if isinstance(lig0.mask_rotate, list) else lig0.mask_rotate)
+        if nb:
+            if mask.shape != (nb, n):
+                raise ValueError(f"mask_rotate of shape {mask.shape} for {nb} rotatable bonds and {n} atoms")
+            if int(rot.min()) < 0 or int(rot.max()) >= n:
+                raise ValueError("rotatable bond outside the ligand")
+            bu.append(rot[:, 0].to(torch.int32))
+            bv.append(rot[:, 1].to(torch.int32))
+            masks.append(torch.from_numpy(mask.astype(np.uint8).reshape(-1)))
+        for d in poses:
+            lig = d['ligand']
+            if int(lig.num_nodes) != n or int(lig.edge_mask.sum()) != nb:
+                raise ValueError("the poses of one complex must have the same atoms and rotatable bonds")
+            rows.append([atom_off, n, bond_off, nb, tor_off, mask_off])
+            atom_off, tor_off = atom_off + n, tor_off + nb
+        bond_off, mask_off = bond_off + nb, mask_off + nb * n
+        max_atoms = max(max_atoms, n)
+    if max(atom_off, tor_off, mask_off) >= 2 ** 31:
+        raise ValueError("packed batch too large for int32 offsets")
+    cat = lambda ts, dt: torch.cat(ts) if ts else torch.zeros(0, dtype=dt)
+    return (torch.tensor(rows, dtype=torch.int32).reshape(-1, 6), cat(bu, torch.int32), cat(bv, torch.int32),
+            cat(masks, torch.uint8), max_atoms)
+
+
+def collate_packed(complexes: List[List[HeteroGraph]], device, non_blocking=True) -> HeteroGraph:
+    """One batch of several complexes: ``complexes`` is a list of pose lists (each what ``sampling`` takes as ``data_list``
+    for one complex).  The result equals ``collate`` of the concatenated pose lists on ``device``, in the given order, with
+    each distinct receptor uploaded once and tiled on the device (``_blocks`` on the receptor store, see
+    ``_collate_receptor_blocks``), and these batch attributes:
+
+    * ``_pose_layout``: ``(layout [n_poses, 6] int32, bond_u, bond_v, mask uint8, max_atoms)`` on the device, the
+      descriptor of ddb200_pose_update_packed (``pose_layout``);
+    * ``_center_node`` [n_poses]: the ligand node pose j of complex c reads in the centre convolution when
+      ``fixed_center_conv=False`` - node ``lig_ptr[first pose of c] + j``, what it reads when its complex is sampled alone;
+    * ``_complex_ptr`` [K + 1] and ``_complex_bond_ptr`` [K + 1]: the pose and rotatable-bond offsets of each complex."""
+    if not complexes or any(len(p) == 0 for p in complexes):
+        raise ValueError("collate_packed takes non-empty pose lists")
+    layout, bu, bv, mask, max_atoms = pose_layout(complexes)
+    out = _collate_receptor_blocks(complexes, device, non_blocking)
+    if out is None:
+        out = collate([d for poses in complexes for d in poses]).to(device, non_blocking=non_blocking)
+    n_poses = [len(p) for p in complexes]
+    pose_ptr = np.concatenate([[0], np.cumsum(n_poses)])
+    first = pose_ptr[:-1]
+    centre = [int(layout[f, 0]) + j for f, n in zip(first, n_poses) for j in range(n)]
+    bond_ptr = [int(layout[f, 4]) for f in first] + [int(layout[-1, 4] + layout[-1, 3])]
+    to = lambda t: t.to(device, non_blocking=non_blocking)
+    out._pose_layout = (to(layout), to(bu), to(bv), to(mask), max_atoms)
+    out._center_node = to(torch.tensor(centre, dtype=torch.long))
+    out._complex_ptr = to(torch.from_numpy(pose_ptr.astype(np.int64)))
+    out._complex_bond_ptr = to(torch.tensor(bond_ptr, dtype=torch.long))
     return out
 
 

@@ -179,7 +179,10 @@ def score_heads(model, data, c, lig_node, tr_sigma, rot_sigma, tor_sigma, sync_f
     c_vec = pos - center[lig.batch]
     c_ea = torch.cat([model.center_distance_expansion(c_vec.norm(dim=-1)), lig.node_sigma_emb], 1)
     c_ea = model.center_edge_embedding(c_ea)
-    idx = arange if model.fixed_center_conv else lig.batch            # hazard C.6: graph id indexes lig_node
+    # hazard C.6: the graph id indexes lig_node.  A packed batch (hetero.collate_packed) gives each pose the node it reads
+    # when its complex is sampled alone
+    centre_node = getattr(data, '_center_node', None)
+    idx = arange if model.fixed_center_conv else (lig.batch if centre_node is None else centre_node[lig.batch])
     c_ea = torch.cat([c_ea, lig_node[idx, :ns]], -1)
     glob = model.final_conv(lig_node, torch.stack([lig.batch, arange]), c_ea, None, out_nodes=B, edge_vec=c_vec,
                             assume_sorted=True)

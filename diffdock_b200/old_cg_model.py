@@ -28,7 +28,8 @@ shape, else ``_forward_host_sized``.  What the v1.0 wiring changes on that path 
 3. The rec<-lig convolution reads ``[ea | node[lig] | node[rec]]`` while its target is the residue: the two node blocks of
    its first Linear are swapped in the kernel plan (TensorProductConvLayer._fused_plan).
 4. rec<-lig uses Y(rec - lig) unnegated (:265): the reverse permutation of the cross list with ``vec_sign = +1``.
-5. Layer-0 rec<-rec messages of a one-receptor, one-time batch are computed for one copy and added to all copies.
+5. Layer-0 rec<-rec messages of a batch of repeated receptors at one time are computed once per distinct receptor and
+   added to all copies.
 
 Confidence mode runs the same sync-free forward with the times as sigmas, then the one-kernel confidence head; where its
 conditions fail it keeps the host-sized forward.
@@ -46,7 +47,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
-from .cg_model import _TABLES, CGModel, _flat, _i32
+from .cg_model import _TABLES, CGModel, _flat, _i32, receptor_tiles
 from .irreps import irreps_str, sh_irreps
 from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_confidence_widths, check_forward, confidence_head,
                      cross_cutoff, cross_graph, edge_weight, ligand_graph, score_heads)
@@ -222,16 +223,12 @@ class CGOldModel(nn.Module):
             return hit[1]
         B, n_lig, ns = data.num_graphs, lig.batch.shape[0], self.ns
         ei = rr.edge_index.long()
-        uniq = getattr(rec, '_unique', None)       # (nodes, edges, copies): the batch holds `copies` identical receptors
-        if uniq is not None and uniq[2] == B and uniq[0] * B == rec.pos.shape[0] and uniq[1] * B == ei.shape[1]:
-            copies, n1, e1 = B, uniq[0], uniq[1]
-        else:
-            copies, n1, e1 = 1, rec.pos.shape[0], ei.shape[1]
-        c = {'copies': copies}
-        # receptor node embedding with the sigma embedding set to zero (:401, :221), one copy, 1280-wide LM layer included
-        x1 = rec.x[:n1].float()
-        base = self.rec_node_embedding(torch.cat([x1, x1.new_zeros((n1, self.sigma_embed_dim))], 1))
-        c['rec_base'] = base.repeat(copies, 1) if copies > 1 else base
+        tiles = receptor_tiles(rec, B, ei)        # copies of the same receptors: each distinct one is embedded once
+        c = {'tiles': tiles}
+        # receptor node embedding with the sigma embedding set to zero (:401, :221), 1280-wide LM layer included
+        x1 = rec.x[tiles['nodes']].float() if tiles is not None else rec.x.float()
+        base = self.rec_node_embedding(torch.cat([x1, x1.new_zeros((x1.shape[0], self.sigma_embed_dim))], 1))
+        c['rec_base'] = base[tiles['node_map']] if tiles is not None else base
         c['rec_sigma_map'] = sigma_map(self.rec_node_embedding, self.sigma_embed_dim, rec.x.shape[1])
         c['rec_gid'] = rec.batch                # complex of each residue: the sigma terms are per complex, not per batch
         # contact graph in CSR order by target (edge_index[0]); vector gathered - target (:406)
@@ -244,11 +241,12 @@ class CGOldModel(nn.Module):
         c['rr_ew'] = _flat(ew)
         c['rr_tgt_batch'] = rec.batch[tgt]
         c['rr_joint'] = (_i32(tgt + n_lig), _i32(src + n_lig))
-        if copies > 1:      # copy 0 of the sorted contact graph (its targets sort first), local numbering
-            c['rr0'] = (_i32(tgt[:e1]), _i32(src[:e1]), vec[:e1].contiguous(),
-                        c['rr_ew'][:e1].contiguous() if c['rr_ew'] is not None else None)
-            c['rr0_row'] = torch.zeros(e1, dtype=torch.int32, device=vec.device)
-            c['rr_perm'] = _i32(torch.arange(ei.shape[1], device=vec.device) % e1)
+        if tiles is not None:   # copy 0 of each distinct receptor's sorted contact graph, numbered as tiles['nodes']
+            rows, shift = tiles['sorted_rows'], tiles['sorted_shift']
+            c['rr0'] = (_i32(tgt[rows] - shift), _i32(src[rows] - shift), vec[rows].contiguous(),
+                        c['rr_ew'][rows].contiguous() if c['rr_ew'] is not None else None)
+            c['rr0_row'] = torch.zeros(rows.shape[0], dtype=torch.int32, device=vec.device)
+            c['rr_perm'] = _i32(tiles['edge_map'])     # sorted row -> copy-0 row (a copy's sorted order is copy 0's)
         c['rec_ptr'] = ops.segment_ptr(rec.batch, B)
         c['lig_ptr'] = ops.segment_ptr(lig.batch, B)
         bonds = ll.edge_index[:, lig.edge_mask].long()
@@ -264,7 +262,7 @@ class CGOldModel(nn.Module):
         constants plus the per-complex sigma terms, four fused convolutions per layer finalised per node type."""
         lig, rec = data['ligand'], data['receptor']
         ns, n_lig, B = self.ns, lig.batch.shape[0], data.num_graphs
-        shared = c['copies'] > 1 and getattr(data, '_uniform_t', False)     # one receptor at one diffusion time
+        shared = c['tiles'] is not None and getattr(data, '_uniform_t', False)     # repeated receptors at one time
         sig = self.timestep_emb_func(data.complex_t['tr'])                    # [B, S], per complex
 
         # -- receptor embeddings (:393-414) -------------------------------------------------------------------------------
@@ -324,15 +322,17 @@ class CGOldModel(nn.Module):
         return layer.batch_norm.fold() if layer.batch_norm is not None else (None, None)
 
     def _shared_receptor_messages(self, x, c, n_lig, ea0, acc):
-        """Layer-0 rec <- rec messages of a batch of B poses of ONE receptor at ONE diffusion time (``data._uniform_t``):
-        the residue features and contact edges (attributes ``ea0`` of copy 0) entering the first layer are the same in
-        every copy, so the messages are computed for copy 0 and added to every copy's rows of ``acc``."""
+        """Layer-0 rec <- rec messages of a batch holding copies of the same receptors at ONE diffusion time
+        (``data._uniform_t``): the residue features and contact edges (attributes ``ea0`` of copy 0) entering the first
+        layer are the same in every copy, so the messages are computed once per distinct receptor, over the concatenated
+        copy-0 graphs, and added to every copy's rows of ``acc``."""
         t0, s0, vec0, ew0 = c['rr0']
-        B, n1 = c['copies'], (x.shape[0] - n_lig) // c['copies']
-        sum0, cnt0 = self.rec_conv_layers[0].accumulate_group(x[n_lig:n_lig + n1], (t0, s0, ea0, vec0, ew0, {}), 0, n1,
-                                                              self.ns)
-        acc[0][n_lig:].view(B, n1, -1).add_(sum0.unsqueeze(0))
-        acc[1][n_lig:].view(B, n1).add_(cnt0.unsqueeze(0))
+        tiles = c['tiles']
+        n_u = tiles['nodes'].shape[0]
+        sum0, cnt0 = self.rec_conv_layers[0].accumulate_group(x[n_lig + tiles['nodes']], (t0, s0, ea0, vec0, ew0, {}), 0,
+                                                              n_u, self.ns)
+        acc[0][n_lig:].add_(sum0[tiles['node_map']])
+        acc[1][n_lig:].add_(cnt0[tiles['node_map']])
 
     def _forward_host_sized(self, data, tr_sigma):
         """Ligand node features after the interaction layers, with exactly-sized neighbour lists (one host read of each

@@ -6,7 +6,8 @@ What each wrapper stands in for in the reference (details per entry point in inc
   radius                                torch_cluster.radius / radius_graph, models/cg_model.py:477,543-548,630
   segment_ptr                           the CSR row pointer of a sorted ``batch`` vector (PyG ``Batch.ptr``)
   pose_update                           utils/sampling.py:133-191 + utils/diffusion_utils.py:60-78 (modify_conformer_batch) +
-                                        utils/torsion.py:75-90 + utils/geometry.py:246-276 (Kabsch)"""
+                                        utils/torsion.py:75-90 + utils/geometry.py:246-276 (Kabsch); pose_update_packed does
+                                        the same for poses of different ligands in one launch"""
 from __future__ import annotations
 
 import ctypes as C
@@ -281,6 +282,35 @@ def pose_update_dev(pos, n_poses, bond_u, bond_v, mask_rotate_u8, tr_score, rot_
                                            C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), _ptr(pose_key),
                                            1 if use_torsion else 0, _ptr(out), _stream())
     _lib.check(rc, 'ddb200_pose_update_dev')
+    PROFILE.all_launches += 1
+    return out
+
+
+def pose_update_packed(pos, layout, max_atoms, bond_u, bond_v, mask_u8, tr_score, rot_score, tor_score, coef_table, err,
+                       step_dev=None, tr_z=None, rot_z=None, tor_z=None, seed=0, pose_key=None, use_torsion=True, out=None):
+    """ddb200_pose_update_packed: ``pose_update_dev`` over poses of different ligands.  ``layout`` [n_poses, 6] int32 on the
+    device (atom_off, n_atoms, bond_off, n_bonds, tor_off, mask_off per pose; include/diffdock_b200.h), ``max_atoms`` >= every
+    pose's n_atoms; ``err`` a device int32 the kernel sets to 1 when a pose is out of range (never reset here).  ``out`` may
+    be ``pos`` itself (in place)."""
+    _need_cuda(pos, layout, tr_score, rot_score, coef_table, err)
+    assert pos.dtype == torch.float32 and pos.is_contiguous() and coef_table.dtype == torch.float32 and coef_table.is_contiguous()
+    assert layout.dtype == torch.int32 and layout.is_contiguous() and layout.dim() == 2 and layout.shape[1] == 6
+    assert err.dtype == torch.int32 and err.numel() >= 1
+    n_poses = layout.shape[0]
+    f = lambda t: t.float().contiguous() if t is not None else None
+    tr_score, rot_score, tor_score, tr_z, rot_z, tor_z = map(f, (tr_score, rot_score, tor_score, tr_z, rot_z, tor_z))
+    if out is None:
+        out = torch.empty_like(pos)
+    if pose_key is not None:
+        assert pose_key.dtype == torch.int64 and pose_key.is_cuda and pose_key.shape[0] >= n_poses
+    if step_dev is not None:
+        assert step_dev.dtype == torch.int32 and step_dev.is_cuda
+    rc = _lib.lib().ddb200_pose_update_packed(_ptr(pos), n_poses, _ptr(layout), int(max_atoms), _ptr(bond_u), _ptr(bond_v),
+                                              _ptr(mask_u8), _ptr(tr_score), _ptr(rot_score), _ptr(tor_score), _ptr(tr_z),
+                                              _ptr(rot_z), _ptr(tor_z), _ptr(coef_table), _ptr(step_dev),
+                                              C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), _ptr(pose_key),
+                                              1 if use_torsion else 0, _ptr(err), _ptr(out), _stream())
+    _lib.check(rc, 'ddb200_pose_update_packed')
     PROFILE.all_launches += 1
     return out
 

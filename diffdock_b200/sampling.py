@@ -18,7 +18,7 @@ import torch
 
 from . import ops
 from .diffusion_utils import set_time
-from .hetero import HeteroGraph, collate, collate_shared_receptor
+from .hetero import HeteroGraph, collate, collate_packed, collate_shared_receptor
 
 
 def randomize_position(data_list, no_torsion, no_random, tr_sigma_max, pocket_knowledge=False, pocket_cutoff=7,
@@ -124,6 +124,34 @@ def _nan_guard(tr, rot, tor):
     return fix(tr), fix(rot), fix(tor)
 
 
+def _nan_guard_packed(tr, rot, tor, pose_ptr, bond_ptr):
+    """``_nan_guard`` per complex of a packed batch, still without a host read: the condition (a NaN in the per-pose mean of
+    the translation score) and ``0.01 * nanmean(|s|)`` are taken over each complex's poses (tr, rot) and bonds (tor), as if
+    it were sampled alone.  ``pose_ptr`` / ``bond_ptr`` [K + 1]: the pose and bond offsets of the complexes (device)."""
+    K = pose_ptr.shape[0] - 1
+    pose_id = torch.searchsorted(pose_ptr[1:], torch.arange(tr.shape[0], device=tr.device), right=True)
+    cond = torch.zeros(K, device=tr.device).index_add_(0, pose_id, torch.isnan(tr.mean(dim=-1)).float()) > 0
+
+    def fix(s, seg):
+        if s is None or s.numel() == 0:
+            return s
+        ids = seg.view((-1,) + (1,) * (s.dim() - 1)).expand_as(s)
+        a = s.abs()
+        ok = ~torch.isnan(a)
+        num = torch.zeros(K, device=s.device, dtype=s.dtype).index_add_(0, ids.reshape(-1), torch.where(ok, a, 0).reshape(-1))
+        den = torch.zeros(K, device=s.device, dtype=s.dtype).index_add_(0, ids.reshape(-1), ok.to(s.dtype).reshape(-1))
+        eps = (0.01 * (num / den))[ids]
+        c = cond[ids]
+        s = torch.where(c & torch.isnan(s), eps, s)
+        s = torch.where(c & (s == float('inf')), eps, s)
+        return torch.where(c & (s == float('-inf')), -eps, s)
+
+    bond_id = None
+    if tor is not None and tor.numel():
+        bond_id = torch.searchsorted(bond_ptr[1:], torch.arange(tor.shape[0], device=tor.device), right=True)
+    return fix(tr, pose_id), fix(rot, pose_id), fix(tor, bond_id)
+
+
 def step_coefficients(t_idx, inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma, model_args, ode,
                       temp_sampling, temp_psi, temp_sigma_data):
     """Host scalars (a, c) per degree of freedom such that  perturbation = a * score + c * z
@@ -223,11 +251,13 @@ class GraphedSteps:
     launches (about 500 kernel launches each) with the host idle."""
 
     def __init__(self, model, g, b, coef_rows, t_rows, bond_u, bond_v, mask_u8, use_torsion, device, draw_noise,
-                 philox=None, warmup=1, consume_warmup=False, crop_rows=None):
+                 philox=None, warmup=1, consume_warmup=False, crop_rows=None, packed=None):
         """``consume_warmup``: when a batch of new shapes needs an eager step before the capture, that step IS step 0 of the
         run (``steps_done`` = 1 afterwards) instead of being thrown away - ``run(n)`` then replays the remaining n - 1.
         ``crop_rows``: the squared receptor-crop cut-off of every step (``crop_cutoff2``); the model then crops the receptor
-        on the device at each step (needs ``model.sync_free_crop_capable()``)."""
+        on the device at each step (needs ``model.sync_free_crop_capable()``).
+        ``packed``: a batch of several complexes (``hetero.collate_packed``; ``bond_u`` / ``bond_v`` / ``mask_u8`` are then
+        unused): the NaN guard runs per complex and the pose update takes each pose's layout from ``g._pose_layout``."""
         self.g, self.b, self.device = g, b, device
         lig = g['ligand']
         self.pos = lig.pos = lig.pos.float().contiguous().clone()         # static buffer, updated in place
@@ -248,8 +278,15 @@ class GraphedSteps:
             g.complex_t = {k: t[i].expand(b) for i, k in enumerate(names)}
             g._uniform_t = True                      # every graph of the batch is at the same diffusion time
             tr, rot, tor = model(g)[:3]
-            tr, rot, tor = _nan_guard(tr, rot, tor)
+            if packed:
+                tr, rot, tor = _nan_guard_packed(tr, rot, tor, g._complex_ptr, g._complex_bond_ptr)
+            else:
+                tr, rot, tor = _nan_guard(tr, rot, tor)
             has_tor = use_torsion and tor is not None and tor.numel() > 0
+            if packed:
+                _pose_update_packed(g, self.pos, tr, rot, tor if has_tor else None, self.coef, self.step, philox, has_tor)
+                self.step.add_(1)
+                return
             tr_z = rot_z = tor_z = None
             if draw_noise and philox is None:
                 tr_z = torch.normal(mean=0, std=1, size=(b, 3), device=device)
@@ -270,7 +307,8 @@ class GraphedSteps:
         if hasattr(model, '_static'):
             model._static(g)
         sig = (b, n_lig, n_rec, int(g['ligand', 'ligand'].edge_index.shape[1]), int(g['receptor', 'receptor'].edge_index.shape[1]),
-               int(bond_u.shape[0]) if bond_u is not None else 0, draw_noise, philox is not None, crop_rows is not None)
+               int(g._pose_layout[1].shape[0]) if packed else int(bond_u.shape[0]) if bond_u is not None else 0, draw_noise,
+               philox is not None, crop_rows is not None)
         seen = getattr(model, '_graph_warmed_shapes', None)
         if seen is None:
             seen = set()
@@ -351,6 +389,14 @@ def _use_cuda_graph(model, model_args, noise_fn, visualization_list, N, batch_si
     return ok
 
 
+def _pose_update_packed(g, pos, tr, rot, tor, coef, step_dev, philox, has_tor):
+    """One in-place ddb200_pose_update_packed step of the packed batch ``g`` (Philox noise keyed by ``philox = (seed,
+    pose keys)``).  Out-of-range poses set ``g._pose_err``, which ``sample_packed`` reads once at the end."""
+    layout, bu, bv, mask, max_atoms = g._pose_layout
+    ops.pose_update_packed(pos, layout, max_atoms, bu, bv, mask, tr, rot, tor, coef, g._pose_err, step_dev=step_dev,
+                           seed=philox[0], pose_key=philox[1], use_torsion=has_tor, out=pos)
+
+
 def crop_cutoff2(t_to_sigma, t_tr, t_rot, t_tor, crop_beyond):
     """The squared receptor-crop cut-off of a step as a float32 value: (3 sigma_tr + crop_beyond)^2 in float64
     (utils/sampling.py:108), rounded as torch rounds a Python float compared with a float32 tensor (utils/utils.py:397)."""
@@ -360,9 +406,10 @@ def crop_cutoff2(t_to_sigma, t_tr, t_rot, t_tor, crop_beyond):
 
 def _eager_steps(g, b, model, inference_steps, tr_schedule, rot_schedule, tor_schedule, t_schedule, t_to_sigma, model_args,
                  coef_rows, device, bond_u, bond_v, mask_u8, use_torsion, ode, no_random, no_final_step_noise, noise_fn,
-                 n_noise, philox, visualization_list, data_list, batch_id, batch_size, n):
+                 n_noise, philox, visualization_list, data_list, batch_id, batch_size, n, packed=False):
     """The step loop launched op by op (utils/sampling.py:96-191): injected noise, per-step receptor cropping, visualisation,
-    or a score model whose shapes are outside the sync-free path."""
+    or a score model whose shapes are outside the sync-free path.  ``packed``: a batch of several complexes
+    (``GraphedSteps``), Philox noise only."""
     coef_dev = torch.tensor(coef_rows, dtype=torch.float32, device=device) if philox else None
     for t_idx in range(inference_steps):
         t_tr, t_rot, t_tor = tr_schedule[t_idx], rot_schedule[t_idx], tor_schedule[t_idx]
@@ -375,9 +422,18 @@ def _eager_steps(g, b, model, inference_steps, tr_schedule, rot_schedule, tor_sc
                  bool(getattr(model_args, 'all_atoms', False)), device)
         mod._uniform_t = True                        # set_time gives every graph of the batch the same diffusion time
         tr_score, rot_score, tor_score = model(mod)[:3]
-        tr_score, rot_score, tor_score = _nan_guard(tr_score, rot_score, tor_score)
+        if packed:
+            tr_score, rot_score, tor_score = _nan_guard_packed(tr_score, rot_score, tor_score, g._complex_ptr,
+                                                               g._complex_bond_ptr)
+        else:
+            tr_score, rot_score, tor_score = _nan_guard(tr_score, rot_score, tor_score)
         has_tor = use_torsion and tor_score.numel() > 0
-        if philox:        # in-kernel counter-based noise: the same draws as the graphed path
+        if packed:
+            step_dev = torch.full((1,), t_idx, dtype=torch.int32, device=device)
+            g['ligand'].pos = g['ligand'].pos.float().contiguous()
+            _pose_update_packed(g, g['ligand'].pos, tr_score, rot_score, tor_score if has_tor else None, coef_dev, step_dev,
+                                philox, has_tor)
+        elif philox:        # in-kernel counter-based noise: the same draws as the graphed path
             step_dev = torch.full((1,), t_idx, dtype=torch.int32, device=device)
             g['ligand'].pos = ops.pose_update_dev(
                 g['ligand'].pos.float().contiguous(), b, bond_u, bond_v, mask_u8, tr_score, rot_score,
@@ -401,6 +457,52 @@ def _eager_steps(g, b, model, inference_steps, tr_schedule, rot_schedule, tor_sc
                 visualization_list[batch_id * batch_size + idx_b].add(
                     (g['ligand'].pos[idx_b * n:n * (idx_b + 1)].detach().cpu()
                      + data_list[batch_id * batch_size + idx_b].original_center.detach().cpu()), part=1, order=t_idx + 2)
+
+
+def _step_tables(inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma, model_args, ode, no_random,
+                 no_final_step_noise, temp_sampling, temp_psi, temp_sigma_data):
+    """``(coef_rows [steps][6], t_rows [steps][3])``: the SDE coefficients (zero noise where the step draws none) and the
+    schedule times of every step."""
+    coef_rows, t_rows = [], []
+    for t_idx in range(inference_steps):
+        coef = step_coefficients(t_idx, inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma,
+                                 model_args, ode, temp_sampling, temp_psi, temp_sigma_data)
+        if ode or no_random or (no_final_step_noise and t_idx == inference_steps - 1):
+            coef[1] = coef[3] = coef[5] = 0.0          # no noise in this step (utils/sampling.py:136-145,158-161)
+        coef_rows.append(coef)
+        t_rows.append([float(tr_schedule[t_idx]), float(rot_schedule[t_idx]), float(tor_schedule[t_idx])])
+    return coef_rows, t_rows
+
+
+def _crop_rows(inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma, model_args):
+    crop_beyond = getattr(model_args, 'crop_beyond', None)
+    return None if crop_beyond is None else [
+        crop_cutoff2(t_to_sigma, tr_schedule[i], rot_schedule[i], tor_schedule[i], crop_beyond)
+        for i in range(inference_steps)]
+
+
+def _rank_batch(confidence_model, confidence_model_args, items, g, pos, b, device):
+    """The confidence of ``b`` final poses (utils/sampling.py:197-227): ``items`` are their confidence graphs and ``pos``
+    their final ligand coordinates; ``items`` None ranks the score batch ``g`` itself."""
+    if items is None:
+        out = confidence_model(g)
+        return out[0] if type(out) is tuple else out
+    crop = getattr(confidence_model_args, 'crop_beyond', None)
+    if isinstance(items[0], HeteroGraph) and not (crop is not None and confidence_model_args.all_atoms):
+        # one receptor copy uploaded and tiled on the device; the collate builds new stores, so the caller's
+        # items are never written to, and the final positions stay on the device
+        cg = collate_shared_receptor(items, device)
+        cg['ligand'].pos = pos.clone()
+    else:
+        cg = collate(copy.deepcopy(items))
+        cg['ligand'].pos = pos.cpu()
+        cg = cg.to(device)
+    if crop is not None:                                                    # utils/sampling.py:213-217
+        cg = crop_receptor(cg, crop)
+    set_time(cg, 0, 0, 0, 0, b, confidence_model_args.all_atoms, device)
+    cg._uniform_t = True                 # every graph of the batch is ranked at t = 0
+    out = confidence_model(cg)
+    return out[0] if type(out) is tuple else out
 
 
 @torch.no_grad()
@@ -446,19 +548,10 @@ def sampling(data_list, model, inference_steps, tr_schedule, rot_schedule, tor_s
         b = g.num_graphs
         n = len(g['ligand'].pos) // b
         keys = keys_all[b0:b0 + b].to(device) if philox else None
-        coef_rows, t_rows = [], []
-        for t_idx in range(inference_steps):
-            coef = step_coefficients(t_idx, inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma,
-                                     model_args, ode, temp_sampling, temp_psi, temp_sigma_data)
-            if ode or no_random or (no_final_step_noise and t_idx == inference_steps - 1):
-                coef[1] = coef[3] = coef[5] = 0.0          # no noise in this step (utils/sampling.py:136-145,158-161)
-            coef_rows.append(coef)
-            t_rows.append([float(tr_schedule[t_idx]), float(rot_schedule[t_idx]), float(tor_schedule[t_idx])])
+        coef_rows, t_rows = _step_tables(inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma, model_args,
+                                         ode, no_random, no_final_step_noise, temp_sampling, temp_psi, temp_sigma_data)
         if graphed and t_schedule is None and b > 0:
-            crop_beyond = getattr(model_args, 'crop_beyond', None)
-            crop_rows = None if crop_beyond is None else [
-                crop_cutoff2(t_to_sigma, tr_schedule[i], rot_schedule[i], tor_schedule[i], crop_beyond)
-                for i in range(inference_steps)]
+            crop_rows = _crop_rows(inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma, model_args)
             steps = GraphedSteps(model, g, b, coef_rows, t_rows, bond_u, bond_v, mask_u8, use_torsion, device,
                                  draw_noise=not (ode or no_random), philox=(seed, keys) if philox else None,
                                  consume_warmup=True, crop_rows=crop_rows)
@@ -471,26 +564,107 @@ def sampling(data_list, model, inference_steps, tr_schedule, rot_schedule, tor_s
         for i in range(b):
             data_list[b0 + i]['ligand'].pos = g['ligand'].pos[i * n:n * (i + 1)]
         if confidence_model is not None:
-            if conf_batches is not None:
-                crop = getattr(confidence_model_args, 'crop_beyond', None)
-                items = conf_batches[batch_id]
-                if isinstance(items[0], HeteroGraph) and not (crop is not None and confidence_model_args.all_atoms):
-                    # one receptor copy uploaded and tiled on the device; the collate builds new stores, so the caller's
-                    # items are never written to, and the final positions stay on the device
-                    cg = collate_shared_receptor(items, device)
-                    cg['ligand'].pos = g['ligand'].pos.clone()
-                else:
-                    cg = collate(copy.deepcopy(items))
-                    cg['ligand'].pos = g['ligand'].pos.cpu()
-                    cg = cg.to(device)
-                if crop is not None:                                                    # utils/sampling.py:213-217
-                    cg = crop_receptor(cg, crop)
-                set_time(cg, 0, 0, 0, 0, b, confidence_model_args.all_atoms, device)
-                cg._uniform_t = True                 # every graph of the batch is ranked at t = 0
-                out = confidence_model(cg)
-            else:
-                out = confidence_model(g)
-            confidence.append(out[0] if type(out) is tuple else out)
+            items = conf_batches[batch_id] if conf_batches is not None else None
+            confidence.append(_rank_batch(confidence_model, confidence_model_args, items, g, g['ligand'].pos, b, device))
     if confidence_model is not None:
         confidence = torch.nan_to_num(torch.cat(confidence, dim=0), nan=-1000)
     return data_list, confidence
+
+
+def pack_plan(costs, max_pairs):
+    """Greedy packing of complexes, in the given order, into batches whose summed cost (poses x ligand atoms x residues, the
+    cross-graph capacity that sets a step's memory) stays within ``max_pairs``; a complex larger than the budget gets a
+    batch of its own.  Returns lists of complex indices."""
+    packs, cur, total = [], [], 0
+    for i, cost in enumerate(costs):
+        if cur and total + cost > max_pairs:
+            packs.append(cur)
+            cur, total = [], 0
+        cur.append(i)
+        total += cost
+    if cur:
+        packs.append(cur)
+    return packs
+
+
+PACK_MAX_PAIRS = 40 * 40 * 1500            # BASELINE config 3 (40 poses x 40 atoms x 1500 residues), a size bench.py runs
+
+
+@torch.no_grad()
+def sample_packed(complexes, model, inference_steps, tr_schedule, rot_schedule, tor_schedule, device, t_to_sigma, model_args,
+                  *, seed, complex_ids=None, no_random=False, ode=False, no_final_step_noise=False, temp_sampling=1.0,
+                  temp_psi=0.0, temp_sigma_data=0.5, confidence_model=None, confidence_data=None,
+                  confidence_model_args=None, max_pairs=None, cuda_graph=None, noise_fn=None, visualization_list=None,
+                  t_schedule=None):
+    """Several docking jobs in one reverse-diffusion step.  ``complexes``: a list of pose lists, each what ``sampling`` takes
+    as ``data_list`` for one complex (``HeteroGraph`` items).  The complexes are packed greedily, in order, into batches of
+    at most ``max_pairs`` poses x ligand atoms x residues (default ``PACK_MAX_PAIRS``; ``pack_plan``); each batch is one
+    ``hetero.collate_packed`` and runs its steps as one captured CUDA graph where ``sampling`` would, else eagerly, with
+    the packed pose update (ddb200_pose_update_packed) and a per-complex NaN guard.  Noise is always Philox, keyed by
+    ``(complex_ids[k] << 32) | pose`` (``complex_ids`` default 0 .. K-1).  ``confidence_data``: one list of confidence graphs
+    per complex, ranked complex by complex with ``sampling``'s code.
+
+    Returns ``[(data_list, confidence)]`` per complex, in input order: what ``sampling(poses, ..., rng='philox',
+    pose_keys=keys, batch_size >= len(poses))`` returns for each complex, up to the summation order of atomics.  The
+    ``fixed_center_conv=False`` centre convolution and the NaN guard behave as for a complex sampled alone."""
+    if noise_fn is not None or visualization_list is not None or t_schedule is not None:
+        raise NotImplementedError("sample_packed draws Philox noise in the pose update: noise_fn, visualization_list and "
+                                  "t_schedule are sampling() options")
+    from .aa_model import AAModel
+    from .old_aa_model import AAOldModel
+    if getattr(model_args, 'all_atoms', False) or isinstance(model, (AAModel, AAOldModel)):
+        raise NotImplementedError("sample_packed runs the coarse-grained score models (CGModel, CGOldModel); all-atom score "
+                                  "models are sampled one complex per sampling() call")
+    device = torch.device(device)
+    if device.type != 'cuda':
+        raise RuntimeError("diffdock_b200.sample_packed runs on a CUDA device only (no CPU fallback)")
+    if confidence_model is not None and confidence_data is None:
+        raise ValueError("sample_packed ranks each complex's confidence graphs: pass confidence_data")
+    K = len(complexes)
+    complex_ids = list(range(K)) if complex_ids is None else [int(i) for i in complex_ids]
+    if len(complex_ids) != K:
+        raise ValueError("one complex id per complex")
+    costs = [len(p) * int(p[0]['ligand'].num_nodes) * int(p[0]['receptor'].num_nodes) for p in complexes]
+    packs = pack_plan(costs, PACK_MAX_PAIRS if max_pairs is None else max_pairs)
+    use_torsion = not model_args.no_torsion
+    graphed = _use_cuda_graph(model, model_args, None, None, 0, 0, cuda_graph)
+    coef_rows, t_rows = _step_tables(inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma, model_args, ode,
+                                     no_random, no_final_step_noise, temp_sampling, temp_psi, temp_sigma_data)
+    crop_rows = _crop_rows(inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma, model_args)
+    results = [None] * K
+    errs = []
+    for pack in packs:
+        g = collate_packed([complexes[k] for k in pack], device)
+        b = g.num_graphs
+        keys = torch.cat([(complex_ids[k] << 32) + torch.arange(len(complexes[k]), dtype=torch.int64) for k in pack])
+        philox = (seed, keys.to(device))
+        g._pose_err = torch.zeros(1, dtype=torch.int32, device=device)
+        errs.append(g._pose_err)
+        if graphed:
+            steps = GraphedSteps(model, g, b, coef_rows, t_rows, None, None, None, use_torsion, device,
+                                 draw_noise=not (ode or no_random), philox=philox, consume_warmup=True, crop_rows=crop_rows,
+                                 packed=True)
+            steps.run(inference_steps)
+        else:
+            _eager_steps(g, b, model, inference_steps, tr_schedule, rot_schedule, tor_schedule, None, t_to_sigma,
+                         model_args, coef_rows, device, None, None, None, use_torsion, ode, no_random, no_final_step_noise,
+                         None, b, philox, None, None, 0, b, 0, packed=True)
+        pos, layout = g['ligand'].pos, g._pose_layout[0].cpu()
+        p0 = 0
+        for k in pack:
+            data_list = complexes[k]
+            for i, d in enumerate(data_list):
+                a0, n = int(layout[p0 + i, 0]), int(layout[p0 + i, 1])
+                d['ligand'].pos = pos[a0:a0 + n]
+            conf = None
+            if confidence_model is not None:
+                a0 = int(layout[p0, 0])
+                a1 = int(layout[p0 + len(data_list) - 1, 0] + layout[p0 + len(data_list) - 1, 1])
+                conf = _rank_batch(confidence_model, confidence_model_args, confidence_data[k], None, pos[a0:a1],
+                                   len(data_list), device)
+                conf = torch.nan_to_num(conf, nan=-1000)
+            results[k] = (data_list, conf)
+            p0 += len(data_list)
+    if errs and int(torch.stack(errs).max()):
+        raise RuntimeError("ddb200_pose_update_packed met a pose outside the declared layout")
+    return results

@@ -125,6 +125,22 @@ int ddb200_pose_update_dev(const float* pos, int64_t n_poses, int n_atoms, int n
                            const float* rot_score, const float* tor_score, const float* tr_z, const float* rot_z,
                            const float* tor_z, const float* coef_table, const int32_t* step_dev, uint64_t seed,
                            const int64_t* pose_key, int use_torsion, float* out_pos, void* stream);
+/* ddb200_pose_update_dev for a batch whose poses belong to different ligands (several complexes sampled in one step).  Row b
+ * of the DEVICE descriptor layout [n_poses, 6] (int32) gives pose b's
+ *   atom_off, n_atoms   its rows of pos / out_pos;
+ *   bond_off, n_bonds   its rows of bond_u / bond_v, in the pose's local atom numbering;
+ *   tor_off             its first entry of tor_score / tor_z (the score model's bond order, pose-major);
+ *   mask_off            the first byte of its [n_bonds, n_atoms] block of the concatenated uint8 masks.
+ * tr_score / rot_score / tr_z / rot_z stay [n_poses, 3].  Coefficients, Philox keys and in-place use as in
+ * ddb200_pose_update_dev.  The host does not read the descriptor: max_atoms (>= every pose's n_atoms) sizes the shared
+ * memory.  A pose with n_atoms outside [1, max_atoms] or a negative n_bonds is left untouched and sets *err (device
+ * int32) to 1; the caller zeroes it and reads it when convenient.  use_torsion needs bond_u, bond_v, mask_rotate and
+ * tor_score. */
+int ddb200_pose_update_packed(const float* pos, int64_t n_poses, const int32_t* layout, int max_atoms, const int32_t* bond_u,
+                              const int32_t* bond_v, const uint8_t* mask_rotate, const float* tr_score,
+                              const float* rot_score, const float* tor_score, const float* tr_z, const float* rot_z,
+                              const float* tor_z, const float* coef_table, const int32_t* step_dev, uint64_t seed,
+                              const int64_t* pose_key, int use_torsion, int32_t* err, float* out_pos, void* stream);
 /* Test hook: the four normals (and optionally the raw 4 x uint32 words) of Philox blocks block0 .. block0 + n_blocks - 1. */
 int ddb200_philox_probe(uint64_t seed, int64_t pose_key, uint32_t step, uint32_t block0, int n_blocks,
                         float* out_normals, uint32_t* out_raw, void* stream);
