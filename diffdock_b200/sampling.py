@@ -251,14 +251,16 @@ class GraphedSteps:
     launches (about 500 kernel launches each) with the host idle."""
 
     def __init__(self, model, g, b, coef_rows, t_rows, bond_u, bond_v, mask_u8, use_torsion, device, draw_noise,
-                 philox=None, warmup=1, consume_warmup=False, crop_rows=None, packed=None):
+                 philox=None, warmup=1, consume_warmup=False, crop_rows=None, packed=None, frames=None):
         """``consume_warmup``: when a batch of new shapes needs an eager step before the capture, that step IS step 0 of the
         run (``steps_done`` = 1 afterwards) instead of being thrown away - ``run(n)`` then replays the remaining n - 1.
         ``crop_rows``: the squared receptor-crop cut-off of every step (``crop_cutoff2``); the model then crops the receptor
         on the device at each step (needs ``model.sync_free_crop_capable()``).
         ``packed``: a batch of several complexes (``hetero.collate_packed``; ``bond_u`` / ``bond_v`` / ``mask_u8`` are then
-        unused): the NaN guard runs per complex and the pose update takes each pose's layout from ``g._pose_layout``."""
-        self.g, self.b, self.device = g, b, device
+        unused): the NaN guard runs per complex and the pose update takes each pose's layout from ``g._pose_layout``.
+        ``frames``: a device buffer [steps, n_atoms of the batch, 3]; every step copies the updated ligand coordinates
+        into its row, indexed by the device step counter."""
+        self.g, self.b, self.device, self.frames = g, b, device, frames
         lig = g['ligand']
         self.pos = lig.pos = lig.pos.float().contiguous().clone()         # static buffer, updated in place
         self.coef = torch.tensor(coef_rows, dtype=torch.float32, device=device).contiguous()        # [steps, 6]
@@ -285,18 +287,19 @@ class GraphedSteps:
             has_tor = use_torsion and tor is not None and tor.numel() > 0
             if packed:
                 _pose_update_packed(g, self.pos, tr, rot, tor if has_tor else None, self.coef, self.step, philox, has_tor)
-                self.step.add_(1)
-                return
-            tr_z = rot_z = tor_z = None
-            if draw_noise and philox is None:
-                tr_z = torch.normal(mean=0, std=1, size=(b, 3), device=device)
-                rot_z = torch.normal(mean=0, std=1, size=(b, 3), device=device)
-                if has_tor:
-                    tor_z = torch.normal(mean=0, std=1, size=tuple(tor.shape), device=device)
-            ops.pose_update_dev(self.pos, b, bond_u, bond_v, mask_u8, tr, rot, tor if has_tor else None, self.coef,
-                                step_dev=self.step, tr_z=tr_z, rot_z=rot_z, tor_z=tor_z,
-                                seed=philox[0] if philox else 0, pose_key=philox[1] if philox else None,
-                                use_torsion=has_tor, out=self.pos)
+            else:
+                tr_z = rot_z = tor_z = None
+                if draw_noise and philox is None:
+                    tr_z = torch.normal(mean=0, std=1, size=(b, 3), device=device)
+                    rot_z = torch.normal(mean=0, std=1, size=(b, 3), device=device)
+                    if has_tor:
+                        tor_z = torch.normal(mean=0, std=1, size=tuple(tor.shape), device=device)
+                ops.pose_update_dev(self.pos, b, bond_u, bond_v, mask_u8, tr, rot, tor if has_tor else None, self.coef,
+                                    step_dev=self.step, tr_z=tr_z, rot_z=rot_z, tor_z=tor_z,
+                                    seed=philox[0] if philox else 0, pose_key=philox[1] if philox else None,
+                                    use_torsion=has_tor, out=self.pos)
+            if frames is not None:
+                frames.index_copy_(0, self.step.long(), self.pos.unsqueeze(0))
             self.step.add_(1)
 
         pos0 = self.pos.clone()
@@ -308,7 +311,7 @@ class GraphedSteps:
             model._static(g)
         sig = (b, n_lig, n_rec, int(g['ligand', 'ligand'].edge_index.shape[1]), int(g['receptor', 'receptor'].edge_index.shape[1]),
                int(g._pose_layout[1].shape[0]) if packed else int(bond_u.shape[0]) if bond_u is not None else 0, draw_noise,
-               philox is not None, crop_rows is not None)
+               philox is not None, crop_rows is not None, frames is not None)
         seen = getattr(model, '_graph_warmed_shapes', None)
         if seen is None:
             seen = set()
@@ -381,11 +384,10 @@ def _use_cuda_graph(model, model_args, noise_fn, visualization_list, N, batch_si
         return False
     crop_ok = getattr(model_args, 'crop_beyond', None) is None or \
         (hasattr(model, 'sync_free_crop_capable') and model.sync_free_crop_capable())
-    ok = (hasattr(model, 'sync_free_capable') and model.sync_free_capable() and noise_fn is None
-          and visualization_list is None and crop_ok)
+    ok = hasattr(model, 'sync_free_capable') and model.sync_free_capable() and noise_fn is None and crop_ok
     if cuda_graph is True and not ok:
-        raise RuntimeError("cuda_graph=True needs the sync-free model path, no noise_fn / visualization, and a model that "
-                           "crops on the device when crop_beyond is set")
+        raise RuntimeError("cuda_graph=True needs the sync-free model path, no noise_fn, and a model that crops on the "
+                           "device when crop_beyond is set")
     return ok
 
 
@@ -406,10 +408,10 @@ def crop_cutoff2(t_to_sigma, t_tr, t_rot, t_tor, crop_beyond):
 
 def _eager_steps(g, b, model, inference_steps, tr_schedule, rot_schedule, tor_schedule, t_schedule, t_to_sigma, model_args,
                  coef_rows, device, bond_u, bond_v, mask_u8, use_torsion, ode, no_random, no_final_step_noise, noise_fn,
-                 n_noise, philox, visualization_list, data_list, batch_id, batch_size, n, packed=False):
-    """The step loop launched op by op (utils/sampling.py:96-191): injected noise, per-step receptor cropping, visualisation,
-    or a score model whose shapes are outside the sync-free path.  ``packed``: a batch of several complexes
-    (``GraphedSteps``), Philox noise only."""
+                 n_noise, philox, frames, packed=False):
+    """The step loop launched op by op (utils/sampling.py:96-191): injected noise, a ``t_schedule``, or a score model whose
+    shapes or cropping are outside the sync-free path.  ``frames``: as for ``GraphedSteps``.  ``packed``: a batch of several
+    complexes (``GraphedSteps``), Philox noise only."""
     coef_dev = torch.tensor(coef_rows, dtype=torch.float32, device=device) if philox else None
     for t_idx in range(inference_steps):
         t_tr, t_rot, t_tor = tr_schedule[t_idx], rot_schedule[t_idx], tor_schedule[t_idx]
@@ -452,11 +454,22 @@ def _eager_steps(g, b, model, inference_steps, tr_schedule, rot_schedule, tor_sc
             coef = list(coef_rows[t_idx])
             g['ligand'].pos = ops.pose_update(g['ligand'].pos, b, bond_u, bond_v, mask_u8, tr_score, rot_score,
                                               tor_score if has_tor else None, coef, tr_z, rot_z, tor_z, use_torsion=has_tor)
-        if visualization_list is not None:
-            for idx_b in range(b):
-                visualization_list[batch_id * batch_size + idx_b].add(
-                    (g['ligand'].pos[idx_b * n:n * (idx_b + 1)].detach().cpu()
-                     + data_list[batch_id * batch_size + idx_b].original_center.detach().cpu()), part=1, order=t_idx + 2)
+        if frames is not None:
+            frames[t_idx].copy_(g['ligand'].pos)
+
+
+def _add_frames(visualization_list, data_list, b0, frames):
+    """Hand the frames of the batch whose first pose is ``b0`` to the caller's visualisation objects (``add(coords, order,
+    part=0, repeat=1)``, utils/visualise.py:PDBFile).  ``frames`` [steps, b, n_atoms, 3] on the host: the ligand
+    coordinates after every step.  Leaves what the reference leaves: frame t + original_center at part 1, order t + 2
+    (utils/sampling.py:193-197), except order 2, which the reference overwrites with each pose's final coordinates once
+    its batch has run (:203-206) - so frame 0 is not kept.  Other entries of the objects are not touched."""
+    steps = frames.shape[0]
+    for i in range(frames.shape[1] if steps else 0):
+        vis, center = visualization_list[b0 + i], data_list[b0 + i].original_center.detach().cpu()
+        vis.add(frames[steps - 1, i] + center, part=1, order=2)
+        for t in range(1, steps):
+            vis.add(frames[t, i] + center, part=1, order=t + 2)
 
 
 def _step_tables(inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma, model_args, ode, no_random,
@@ -550,22 +563,26 @@ def sampling(data_list, model, inference_steps, tr_schedule, rot_schedule, tor_s
         keys = keys_all[b0:b0 + b].to(device) if philox else None
         coef_rows, t_rows = _step_tables(inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma, model_args,
                                          ode, no_random, no_final_step_noise, temp_sampling, temp_psi, temp_sigma_data)
+        frames = None
+        if visualization_list is not None:
+            frames = torch.empty((inference_steps, b * n, 3), dtype=torch.float32, device=device)
         if graphed and t_schedule is None and b > 0:
             crop_rows = _crop_rows(inference_steps, tr_schedule, rot_schedule, tor_schedule, t_to_sigma, model_args)
             steps = GraphedSteps(model, g, b, coef_rows, t_rows, bond_u, bond_v, mask_u8, use_torsion, device,
                                  draw_noise=not (ode or no_random), philox=(seed, keys) if philox else None,
-                                 consume_warmup=True, crop_rows=crop_rows)
+                                 consume_warmup=True, crop_rows=crop_rows, frames=frames)
             steps.run(inference_steps)
         else:
             _eager_steps(g, b, model, inference_steps, tr_schedule, rot_schedule, tor_schedule, t_schedule, t_to_sigma,
                          model_args, coef_rows, device, bond_u, bond_v, mask_u8, use_torsion, ode, no_random,
-                         no_final_step_noise, noise_fn, min(batch_size, N), (seed, keys) if philox else None,
-                         visualization_list, data_list, batch_id, batch_size, n)
+                         no_final_step_noise, noise_fn, min(batch_size, N), (seed, keys) if philox else None, frames)
         for i in range(b):
             data_list[b0 + i]['ligand'].pos = g['ligand'].pos[i * n:n * (i + 1)]
         if confidence_model is not None:
             items = conf_batches[batch_id] if conf_batches is not None else None
             confidence.append(_rank_batch(confidence_model, confidence_model_args, items, g, g['ligand'].pos, b, device))
+        if frames is not None:                   # one device->host copy per batch
+            _add_frames(visualization_list, data_list, b0, frames.view(inference_steps, b, n, 3).cpu())
     if confidence_model is not None:
         confidence = torch.nan_to_num(torch.cat(confidence, dim=0), nan=-1000)
     return data_list, confidence
@@ -648,7 +665,7 @@ def sample_packed(complexes, model, inference_steps, tr_schedule, rot_schedule, 
         else:
             _eager_steps(g, b, model, inference_steps, tr_schedule, rot_schedule, tor_schedule, None, t_to_sigma,
                          model_args, coef_rows, device, None, None, None, use_torsion, ode, no_random, no_final_step_noise,
-                         None, b, philox, None, None, 0, b, 0, packed=True)
+                         None, b, philox, None, packed=True)
         pos, layout = g['ligand'].pos, g._pose_layout[0].cpu()
         p0 = 0
         for k in pack:
