@@ -408,3 +408,75 @@ def canonical_contact_edges(edge_index, coords):
             out[0, start:end] = nb[order]
         start = end
     return out
+
+
+CONTACT_CAP = 1024        # hits contact_kernel (csrc/inputs.cu) keeps per centre in shared memory
+
+
+class ContactRule:
+    """The contact graph's documented rule (diffdock_b200.inputs.contact_graph), vectorised so that it runs at the
+    3000-residue limit: the distances of oracle.inputs.cdist_f32 (torch.cdist's fp32 arithmetic, direct form up to 25
+    points), one stable argsort per row - every exact distance tie broken by index - and the centre excluded by index, not
+    by distance (a duplicate of the centre, d = 0 with j != i, is an ordinary neighbour).  Per centre, with
+    hits = #{j != i : d_ij < cutoff}:
+        knn_only     the min(K, n - 1) nearest by (distance, index)
+        hits == 0    the nearest other point (none when n == 1)
+        hits <= K    the hits in index order
+        hits >  K    the K nearest by (distance, index)
+    K = max_neighbors or 1000.  Distances and order depend on the points only, so one instance serves every cut-off and K."""
+
+    def __init__(self, coords):
+        from oracle.inputs import cdist_f32
+        self.d = cdist_f32(coords)
+        self.n = self.d.shape[0]
+        self._order = None
+
+    @property
+    def order(self):
+        """[n, n - 1]: every centre's other points by (distance, index)."""
+        if self._order is None:
+            import numpy as np
+            o = np.argsort(self.d, axis=1, kind='stable')
+            self._order = o[o != np.arange(self.n)[:, None]].reshape(self.n, self.n - 1)
+        return self._order
+
+    def graph(self, cutoff, max_neighbors=None, knn_only=False):
+        """(edge_index [2, E] int64, rows [neighbour, centre], listed centre by centre; hits [n] as contact_kernel counts
+        them: the points within the cut-off, or all n - 1 others when ``knn_only``)."""
+        import numpy as np
+        n, k = self.n, (max_neighbors if max_neighbors else 1000)
+        hit = self.d < np.float32(cutoff)
+        np.fill_diagonal(hit, False)
+        hits = np.full(n, n - 1) if knn_only else hit.sum(1)
+        rows = []
+        for i in range(n):
+            if knn_only:
+                rows.append(self.order[i, :min(k, n - 1)])
+            elif hits[i] == 0:
+                rows.append(self.order[i, :1])
+            elif hits[i] <= k:
+                rows.append(np.flatnonzero(hit[i]))
+            else:
+                rows.append(self.order[i, :k])
+        nbr = np.concatenate(rows) if rows else np.zeros(0, np.int64)
+        ctr = np.repeat(np.arange(n), [len(r) for r in rows])
+        return np.stack([nbr, ctr]).astype(np.int64).reshape(2, -1), hits
+
+
+def contact_paths(hits, max_neighbors=None, knn_only=False):
+    """Per centre, the branch of contact_kernel that writes its row, from the rule's hit counts (knn_only: hits = n - 1):
+        'list_index'     0 < hits <= K, hits <= CAP     the shared-memory hit list, index order
+        'rescan_index'   CAP < hits <= K                a second scan of all points, index order
+        'list_select'    hits > K, hits <= CAP          K selection rounds over the list
+        'rescan_select'  hits > K, hits > CAP           K selection rounds, each rescanning all points with the cut-off
+        'nearest'        hits == 0                      nearest other point, by a full rescan
+        'knn_list'       knn_only, n - 1 <= CAP         selection over the list
+        'knn_rescan'     knn_only, n - 1 > CAP          selection by full rescans"""
+    import numpy as np
+    hits = np.asarray(hits)
+    k = max_neighbors if max_neighbors else 1000
+    if knn_only:
+        return np.where(hits <= CONTACT_CAP, 'knn_list', 'knn_rescan')
+    small = hits <= CONTACT_CAP
+    return np.select([hits == 0, (hits <= k) & small, hits <= k, small],
+                     ['nearest', 'list_index', 'rescan_index', 'list_select'], 'rescan_select')

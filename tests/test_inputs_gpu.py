@@ -33,10 +33,13 @@ def test_contact_graph_matches_reference(built_lib, fx, i):
     assert torch.equal(g['receptor'].x.cpu(), c['x']) and torch.equal(g['receptor'].pos.cpu(), c['pos'])
 
 
-@pytest.mark.parametrize('n,cutoff,k', [(2500, 15.0, 24), (700, 40.0, 1000), (900, 3.0, 5), (1, 5.0, 3), (2, 0.5, 3)])
+@pytest.mark.parametrize('n,cutoff,k', [(2500, 15.0, 24), (700, 40.0, 1000), (1400, 60.0, 1500), (900, 3.0, 5), (1, 5.0, 3),
+                                        (2, 0.5, 3)])
 def test_contact_graph_matches_oracle(built_lib, n, cutoff, k):
-    """Sizes and regimes the fixture does not hold: a large receptor, every hit kept in index order with more hits than the
-    shared-memory list holds (cut-off 40 A, K = 1000), mostly isolated points (nearest-other rule), degenerate sizes."""
+    """Sizes and regimes the fixture does not hold: a large receptor, every hit kept in index order from the shared-memory
+    list (700 points, cut-off 40 A, K = 1000: at most 699 hits, within the list's 1024), every hit kept in index order with
+    more hits than the list holds (1400 points, 60 A, K = 1500: the kernel rescans), mostly isolated points (nearest-other
+    rule), degenerate sizes.  tests/test_contact_graph_ref_gpu.py covers the rescan paths at the list's capacity."""
     from oracle.inputs import contact_graph as oracle_graph
     from diffdock_b200.inputs import contact_graph
     rng = np.random.default_rng(n)
