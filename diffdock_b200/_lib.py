@@ -42,7 +42,8 @@ SIGNATURES = {
     'ddb200_contact_count': (_int, [_vp, _i32, C.c_float, _i32, _i32, _vp, _vp]),
     'ddb200_contact_fill': (_int, [_vp, _i32, C.c_float, _i32, _i32, _vp, _vp, _vp, _vp]),
     'ddb200_crop_flags': (_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
-    'ddb200_crop_select_edges': (_int, [_vp, _vp, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'ddb200_crop_select_edges': (_int, [_vp, _vp, _vp, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'ddb200_receptor_need': (_int, [_vp, _vp, _i64, _i32, _vp, _vp, _i64, _vp, _i64, _i32, _vp, _vp]),
     'ddb200_confidence_head': (_int, [_vp, _i64, _i64, _vp, _i32, _i32, _i32, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _i32,
                                       _vp, _vp, _vp]),
 }

@@ -145,6 +145,9 @@ class CGModel(nn.Module):
             self.lig_emb_layers = nn.ModuleList([self.conv(i, 1) for i in range(num_prot_emb_layers)])
         self.conv_layers = self._interaction_stack(4, 2)
         self._sync_free = None
+        # the sync-free forward drops receptor <- receptor messages that cannot reach a ligand atom (_pruned_contact_groups);
+        # False runs every contact edge in every layer, for comparisons only
+        self._prune_receptor = True
         if confidence_mode:
             self._confidence_heads(confidence_dropout, confidence_no_batchnorm, num_confidence_outputs)
             return
@@ -353,14 +356,18 @@ class CGModel(nn.Module):
                                "batch cannot take (more than 10000 residues in a complex)")
         return self._forward_host_sized(data, c)
 
-    def _interaction_layers(self, node, groups, n_last, merge=False, shared=None):
+    def _interaction_layers(self, node, groups, n_last, merge=False, shared=None, per_layer=None):
         """The interaction layers over the joint graph; the last one only takes the first ``n_last`` groups, the edges that
         end on ligand atoms (models/cg_model.py:347-349).  ``merge``: one radial MLP for all edge types runs them as a
         single group (exactly-sized lists only).  ``shared = (accumulators, k)``: layer 0 starts from messages computed
-        elsewhere instead of running group ``k``."""
+        elsewhere instead of running group ``k``.  ``per_layer = (k, [group | None per layer])``: layer l runs the given
+        group in place of group ``k`` where one is given."""
         L = len(self.conv_layers)
         for l, layer in enumerate(self.conv_layers):
             use, init = (groups if l < L - 1 else groups[:n_last]), None
+            if per_layer is not None and per_layer[1][l] is not None:
+                k = per_layer[0]
+                use = use[:k] + [per_layer[1][l]] + use[k + 1:]
             if l == 0 and shared is not None:
                 init, skip = shared
                 use = use[:skip] + [None] + use[skip + 1:]
@@ -383,13 +390,15 @@ class CGModel(nn.Module):
         # -- embeddings (models/cg_model.py:272-306) --------------------------------------------------------------
         sig = self.rec_sigma_embedding(self.timestep_emb_func(data.complex_t['tr'])).contiguous()      # [B, ns]
         crop = getattr(data, '_crop', None)
+        prune = self._prune_receptor and len(self.conv_layers) > 1
+        keep = None
         if crop is None:
             rec_node, rec_pos = rec.rec_node_attr.clone(), rec.pos.float().contiguous()
             rr_tgt32 = _rr_joint(c, n_lig)
             g_rr = (rr_tgt32[0], rr_tgt32[1], c['rr_ea'], c['rr_vec'], _flat(c['rr_ew']),
                     dict(ea_add=sig, ea_add_idx=c['rr_gid32']))
         else:
-            rec_node, rec_pos, g_rr = self._cropped_receptor(data, c, crop, sig, n_lig)
+            rec_node, rec_pos, g_rr, keep = self._cropped_receptor(data, c, crop, sig, n_lig, select=not prune)
         rec_node[:, :ns] += sig[rec.batch]
         lig_node, g_ll = self._ligand_graph_sync_free(data, c)
 
@@ -408,14 +417,58 @@ class CGModel(nn.Module):
         # the shared layer-0 messages assume every pose keeps every residue
         shared = self._shared_receptor_messages(data, c, rec, rec_node, sig, n_lig) \
             if len(self.conv_layers) > 1 and crop is None else None
-        node = self._interaction_layers(node, groups, 2, shared=(shared, 2) if shared is not None else None)
+        pruned = self._pruned_contact_groups(c, g_rl, keep, sig, n_lig, rec_node.shape[0], shared is not None) \
+            if prune else None
+        node = self._interaction_layers(node, groups, 2, shared=(shared, 2) if shared is not None else None,
+                                        per_layer=(2, pruned) if pruned is not None else None)
         return self._heads(data, c, node[:n_lig], tr_sigma, rot_sigma, tor_sigma, sync_free=True)
 
-    def _cropped_receptor(self, data, c, crop, sig, n_lig):
+    def _need_levels(self, L, shared):
+        """Per interaction layer l, the k of the need set R_k its receptor <- receptor group is restricted to, or None: the
+        last layer has no such group, and layer 0 keeps the shared messages when they apply.  Layer l's output reaches the
+        ligand through L - 1 - l more layers, one contact hop each, the last of which ends on ligand atoms."""
+        return [None if l == L - 1 or (l == 0 and shared) else L - 1 - l for l in range(L)]
+
+    def _pruned_contact_groups(self, c, g_rl, keep, sig, n_lig, n_rec, shared):
+        """The receptor <- receptor group of every interaction layer restricted to targets that can still pass a message to
+        a ligand atom (None where the layer keeps its group).  Only the ligand's final features reach the outputs, so a
+        residue's features after layer l matter only through a chain of messages into the ligand in layers l+1 .. L-1:
+        R_1 = the targets of this step's receptor <- ligand edges (g_rl, the edges the convolutions use), R_{k+1} = R_k and
+        the sources of the contact edges into R_k (under a crop, only the edges whose two ends are kept), and layer l needs
+        its targets in R_{L-1-l}.
+
+        Invariant: a residue outside layer l's set gets no contact messages in that layer, so its row of the layer output
+        is wrong, and no later layer or head reads it - the contact and receptor -> ligand messages of later layers only
+        gather from R_{L-1-l} (the ligand graph, the cross groups and the heads never see other residues).  Every buffer
+        lives in ``c``, so a captured step allocates nothing."""
+        levels = self._need_levels(len(self.conv_layers), shared)
+        n_levels = max((k for k in levels if k is not None), default=0)
+        if n_levels == 0:
+            return None
+        if 'rr_tgt32l' not in c:
+            c['rr_tgt32l'] = (_i32(c['rr_tgt']), _i32(c['rr_src']))
+        tgt32, src32 = c['rr_tgt32l']
+        key = ('prune', n_lig, n_levels)
+        if key not in c:
+            c[key] = (torch.empty((n_levels, n_rec), dtype=torch.uint8, device=tgt32.device),
+                      [ops.select_edges_buffers(tgt32.shape[0], tgt32.device) for _ in range(n_levels)])
+        need_buf, bufs = c[key]
+        need = ops.receptor_need(g_rl[0], g_rl[5]['n_edges_dev'], n_lig, tgt32, src32, n_rec, n_levels, keep=keep,
+                                 out=need_buf)
+        ew, sel = _flat(c['rr_ew']), {}
+        for k in sorted({k for k in levels if k is not None}):
+            t, s_, perm, gid, n_dev = ops.crop_select_edges(tgt32, src32, keep, c['rr_gid32'], offset=n_lig,
+                                                            need=need[k - 1], out=bufs[k - 1])
+            sel[k] = (t, s_, c['rr_ea'], c['rr_vec'], ew,
+                      dict(n_edges_dev=n_dev, edge_perm=perm, ea_add=sig, ea_add_idx=gid))
+        return [sel[k] if k is not None else None for k in levels]
+
+    def _cropped_receptor(self, data, c, crop, sig, n_lig, select=True):
         """utils/sampling.py:104-109 in masked form: the residues farther than the step's cut-off from every ligand atom of
         their complex keep their rows but lose every edge.  ``crop = (cutoff2_table, step_dev)``.  Returns the receptor node
         features (the embedding layers rerun over the cropped contact graph, as the reference embeds its cropped batch),
-        the positions for the cross-graph search (+inf at dropped residues) and the rec <- rec edge group."""
+        the positions for the cross-graph search (+inf at dropped residues), the rec <- rec edge group (None when
+        ``select`` is False and no embedding layer needs it: the pruned layers select their own) and the keep flags."""
         if not self.sync_free_crop_capable():
             raise RuntimeError("per-step receptor cropping needs every receptor embedding layer on the fused kernel "
                                "(CGModel.sync_free_crop_capable)")
@@ -424,6 +477,8 @@ class CGModel(nn.Module):
                                        c['rec_batch32'], crop[0], crop[1])
         if 'rr_tgt32l' not in c:
             c['rr_tgt32l'] = (_i32(c['rr_tgt']), _i32(c['rr_src']))
+        if not select and not len(self.rec_emb_layers):
+            return rec.rec_node_attr.clone(), rec_pos, None, keep
         tgt, src, perm, gid, n_dev = ops.crop_select_edges(*c['rr_tgt32l'], keep, c['rr_gid32'], offset=n_lig)
         ew = _flat(c['rr_ew'])
         if len(self.rec_emb_layers):
@@ -434,7 +489,7 @@ class CGModel(nn.Module):
         else:
             node = rec.rec_node_attr.clone()
         g_rr = (tgt, src, c['rr_ea'], c['rr_vec'], ew, dict(n_edges_dev=n_dev, edge_perm=perm, ea_add=sig, ea_add_idx=gid))
-        return node, rec_pos, g_rr
+        return node, rec_pos, g_rr, keep
 
     def _ligand_graph_sync_free(self, data, c):
         """Bonds + radius graph, CSR by target, built on the device (models/cg_model.py:467-497), and the ligand embedding

@@ -334,30 +334,65 @@ def crop_flags(lig_pos, lig_ptr, rec_pos, rec_batch32, cutoff2_table, step_dev=N
     return keep, masked
 
 
-def crop_select_edges(tgt32, src32, keep, gid32=None, offset=0):
-    """The edges of a static list whose two ends are kept, original order (ddb200_crop_select_edges): ``(tgt + offset,
-    src + offset, perm, gid | None, n_dev)`` in buffers as long as the input; only the first ``n_dev[0]`` rows are live.
-    No host synchronisation."""
-    _need_cuda(tgt32, src32, keep)
+def crop_select_edges(tgt32, src32, keep, gid32=None, offset=0, need=None, out=None):
+    """The edges of a static list whose two ends are kept and whose target is needed, original order
+    (ddb200_crop_select_edges): ``(tgt + offset, src + offset, perm, gid | None, n_dev)`` in buffers as long as the input;
+    only the first ``n_dev[0]`` rows are live.  ``keep`` / ``need`` (bool / uint8 [n_rec]): None drops that condition.
+    ``out``: buffers of an earlier call with the same list to write into (``select_edges_buffers``), so that a captured
+    step allocates nothing.  No host synchronisation."""
+    _need_cuda(tgt32, src32, keep, need)
     assert tgt32.dtype == torch.int32 and src32.dtype == torch.int32 and tgt32.is_contiguous() and src32.is_contiguous()
-    assert keep.dtype == torch.bool and keep.is_contiguous()
+    for f in (keep, need):
+        if f is not None:
+            assert f.dtype in (torch.bool, torch.uint8) and f.is_contiguous()
     if gid32 is not None:
         assert gid32.dtype == torch.int32 and gid32.is_contiguous()
-    n, dev = tgt32.shape[0], tgt32.device
-    L = _lib.lib()
-    need = C.c_size_t(0)
-    _lib.check(L.ddb200_crop_select_edges(None, None, None, n, None, 0, None, None, None, None, None, None, C.byref(need),
-                                          _stream()), 'ddb200_crop_select_edges(size)')
-    ws = torch.empty(max(int(need.value), 1), dtype=torch.uint8, device=dev)
-    out_t, out_s, perm = (torch.empty(max(n, 1), dtype=torch.int32, device=dev) for _ in range(3))
-    out_g = torch.empty(max(n, 1), dtype=torch.int32, device=dev) if gid32 is not None else None
-    n_dev = torch.empty(1, dtype=torch.int32, device=dev)
+    n = tgt32.shape[0]
+    if out is None:
+        out = select_edges_buffers(n, tgt32.device, gid32 is not None)
+    ws, out_t, out_s, perm, out_g, n_dev = out
+    assert out_t.shape[0] >= n and (out_g is not None or gid32 is None)
     have = C.c_size_t(ws.numel())
-    _lib.check(L.ddb200_crop_select_edges(_ptr(tgt32), _ptr(src32), _ptr(gid32), n, _ptr(keep), int(offset), _ptr(out_t),
-                                          _ptr(out_s), _ptr(perm), _ptr(out_g), _ptr(n_dev), _ptr(ws), C.byref(have),
-                                          _stream()), 'ddb200_crop_select_edges')
+    _lib.check(_lib.lib().ddb200_crop_select_edges(_ptr(tgt32), _ptr(src32), _ptr(gid32), n, _ptr(keep), _ptr(need),
+                                                   int(offset), _ptr(out_t), _ptr(out_s), _ptr(perm),
+                                                   _ptr(out_g if gid32 is not None else None), _ptr(n_dev), _ptr(ws),
+                                                   C.byref(have), _stream()), 'ddb200_crop_select_edges')
     PROFILE.all_launches += 4
-    return out_t[:n], out_s[:n], perm[:n], out_g[:n] if out_g is not None else None, n_dev
+    return out_t[:n], out_s[:n], perm[:n], out_g[:n] if gid32 is not None else None, n_dev
+
+
+def select_edges_buffers(n, dev, with_gid=True):
+    """Workspace and outputs of ``crop_select_edges`` over a list of ``n`` edges: ``(workspace, tgt, src, perm, gid | None,
+    n_dev)``."""
+    L = _lib.lib()
+    size = C.c_size_t(0)
+    _lib.check(L.ddb200_crop_select_edges(None, None, None, n, None, None, 0, None, None, None, None, None, None,
+                                          C.byref(size), _stream()), 'ddb200_crop_select_edges(size)')
+    ws = torch.empty(max(int(size.value), 1), dtype=torch.uint8, device=dev)
+    out_t, out_s, perm = (torch.empty(max(n, 1), dtype=torch.int32, device=dev) for _ in range(3))
+    out_g = torch.empty(max(n, 1), dtype=torch.int32, device=dev) if with_gid else None
+    return ws, out_t, out_s, perm, out_g, torch.empty(1, dtype=torch.int32, device=dev)
+
+
+def receptor_need(cross_tgt32, n_cross, offset, tgt32, src32, n_rec, n_levels, keep=None, out=None):
+    """The residues that can still pass a message to a ligand atom (ddb200_receptor_need): uint8 [n_levels, n_rec], row k
+    = R_{k+1}.  R_1: ``cross_tgt32[e] - offset`` for e < ``n_cross[0]`` (the receptor <- ligand edges in the joint
+    numbering, a capacity buffer); each further row adds the sources of the contact edges ``tgt32`` / ``src32`` (receptor
+    numbering) into the previous one, over edges whose two ends are kept (``keep`` None: all).  No host synchronisation."""
+    _need_cuda(cross_tgt32, n_cross, tgt32, src32, keep)
+    for t in (cross_tgt32, n_cross, tgt32, src32):
+        assert t.dtype == torch.int32 and t.is_contiguous()
+    if keep is not None:
+        assert keep.dtype in (torch.bool, torch.uint8) and keep.is_contiguous() and keep.shape[0] == n_rec
+    if out is None:
+        out = torch.empty((n_levels, n_rec), dtype=torch.uint8, device=tgt32.device)
+    assert out.dtype == torch.uint8 and out.is_contiguous() and out.shape == (n_levels, n_rec)
+    rc = _lib.lib().ddb200_receptor_need(_ptr(cross_tgt32), _ptr(n_cross), cross_tgt32.shape[0], int(offset), _ptr(tgt32),
+                                         _ptr(src32), tgt32.shape[0], _ptr(keep), int(n_rec), int(n_levels), _ptr(out),
+                                         _stream())
+    _lib.check(rc, 'ddb200_receptor_need')
+    PROFILE.all_launches += max(n_levels, 0)
+    return out
 
 
 CONF_MAX_IN, CONF_MAX_HIDDEN, CONF_MAX_OUT = 256, 128, 16       # DDB200_CONF_MAX_* of include/diffdock_b200.h

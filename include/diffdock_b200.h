@@ -296,20 +296,33 @@ int ddb200_contact_fill(const float* pos, int32_t n, float cutoff, int32_t max_n
  *   rec_pos_masked [n_rec, 3] = rec_pos, with +inf in every coordinate of a dropped residue (handed to the radius kernels
  *   as candidates or queries, a dropped residue then has no neighbour: d^2 < r^2 is false).
  * ddb200_crop_select_edges: the edges e of a static list (tgt / src [n_edges] receptor indices, gid [n_edges] any int32
- *   payload, may be NULL together with out_gid) with keep[tgt[e]] && keep[src[e]], in their original order:
+ *   payload, may be NULL together with out_gid) with keep[tgt[e]] && keep[src[e]] && need[tgt[e]] (keep NULL / need NULL:
+ *   that condition holds for every edge), in their original order:
  *   out_perm[k] = e, out_tgt[k] = tgt[e] + offset, out_src[k] = src[e] + offset, out_gid[k] = gid[e] for k < *n_selected;
  *   the output arrays have n_edges rows, rows at and beyond *n_selected are unspecified; the count stays in device memory.
  *   Workspace protocol as ddb200_csr_sort_by_target (workspace == NULL: size query).
  * Replaces: utils/utils.py:388-413 (crop_beyond, all_atoms=False) as called at utils/sampling.py:104-109, without the
  * deep copy / to_data_list / re-collate of the batch.
  * ------------------------------------------------------------------------------------------------------------- */
+/* ---------------------------------------------------------------------------------------------------------------
+ * ddb200_receptor_need: the residues whose features after an interaction layer can still reach a ligand atom.
+ *   need [n_levels, n_rec] bytes (0 / 1), row k = R_{k+1}:
+ *   R_1     = { cross_tgt[e] - offset : e < min(*n_cross, cross_cap) }   (the targets of the step's receptor <- ligand
+ *             edges in the joint numbering; offset = number of ligand atoms)
+ *   R_{k+1} = R_k | { src[e] : tgt[e] in R_k, and keep[tgt[e]] && keep[src[e]] (keep NULL: every edge) }
+ *   over the static contact list tgt / src [n_edges] (receptor indices).  One memset, one seed launch and one launch per
+ *   further level; no host value is read, so the call can be captured in a CUDA graph.
+ * ------------------------------------------------------------------------------------------------------------- */
 int ddb200_crop_flags(const float* lig_pos, const int32_t* lig_ptr, const float* rec_pos, const int32_t* rec_batch,
                       int64_t n_rec, const float* cutoff2_table, const int32_t* step_dev, uint8_t* keep,
                       float* rec_pos_masked, void* stream);
 int ddb200_crop_select_edges(const int32_t* tgt, const int32_t* src, const int32_t* gid, int64_t n_edges,
-                             const uint8_t* keep, int32_t offset, int32_t* out_tgt, int32_t* out_src, int32_t* out_perm,
-                             int32_t* out_gid, int32_t* n_selected, void* workspace, size_t* workspace_bytes,
-                             void* stream);
+                             const uint8_t* keep, const uint8_t* need, int32_t offset, int32_t* out_tgt, int32_t* out_src,
+                             int32_t* out_perm, int32_t* out_gid, int32_t* n_selected, void* workspace,
+                             size_t* workspace_bytes, void* stream);
+int ddb200_receptor_need(const int32_t* cross_tgt, const int32_t* n_cross, int64_t cross_cap, int32_t offset,
+                         const int32_t* tgt, const int32_t* src, int64_t n_edges, const uint8_t* keep, int64_t n_rec,
+                         int32_t n_levels, uint8_t* need, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * ddb200_confidence_head: the confidence head of the confidence models, one CTA per pose b, atoms lig_ptr[b] ..
