@@ -23,7 +23,7 @@ import torch
 from torch import nn
 
 from . import ops
-from .cg_model import CGModel, _i32
+from .cg_model import CGModel, _i32, linked_edge_tiles, receptor_tiles
 from .layers import AtomEncoder, _mlp, cross_cutoff, cross_graph
 from .synthetic import REC_ATOM_FEATURE_DIMS as rec_atom_feature_dims
 
@@ -95,10 +95,25 @@ class AAModel(CGModel):
         t32, order, _ = ops.csr_sort_by_target(_i32(tgt), n_rows)
         return (t32, _i32(src[order])) + tuple(p[order].contiguous() for p in payload)
 
+    @staticmethod
+    def _receptor_tiles(data, B, rr_ei, aa_ei, ar_ei):
+        """Index maps between a batch whose residue and atom stores carry a block layout (``_blocks`` / ``_unique``) and its
+        distinct receptors: ``{'rec': .., 'atom': ..}`` from ``receptor_tiles``, ``'ar'`` from ``linked_edge_tiles`` for the
+        atom-residue edges; None without a layout."""
+        rt = receptor_tiles(data['receptor'], B, rr_ei)
+        at = receptor_tiles(data['atom'], B, aa_ei) if rt is not None else None
+        lt = linked_edge_tiles(data['atom'], at, rt, ar_ei, B) if at is not None else None
+        return None if lt is None else dict(rec=rt, atom=at, ar=lt)
+
     def _static(self, data):
         """Pose-independent part, cached on ``data`` like models/aa_model.py:276-333: residue / atom node embeddings, the
         edge embeddings of the three static graphs (residue-residue, atom-atom, atom-residue), the optional protein
-        embedding layers over their four groups, and the CSR-sorted static edge groups of the joint graph."""
+        embedding layers over their four groups, and the CSR-sorted static edge groups of the joint graph.
+
+        When the batch holds copies of the same receptors (the poses of one complex, ``collate_shared_receptor``, or several
+        complexes of a packed batch, ``collate_packed``), the embeddings and the protein embedding layers run once per
+        distinct receptor and are mapped onto the batch rows; the reference recomputes them for every pose
+        (models/aa_model.py:276-333 over the B-fold receptor)."""
         rec, atom, lig = data['receptor'], data['atom'], data['ligand']
         rr, aa, ar, ll = data['receptor', 'receptor'], data['atom', 'atom'], data['atom', 'receptor'], data['ligand', 'ligand']
         if hasattr(rec, 'rec_node_attr') and hasattr(rr, '_b200aa'):
@@ -109,21 +124,39 @@ class AAModel(CGModel):
         rr_ei, aa_ei, ar_ei = rr.edge_index.long(), aa.edge_index.long(), ar.edge_index.long()
         rr_vec, aa_vec = rp[rr_ei[1]] - rp[rr_ei[0]], ap[aa_ei[1]] - ap[aa_ei[0]]
         ar_vec = rp[ar_ei[1]] - ap[ar_ei[0]]
-        rr_ea = self.rec_edge_embedding(self.rec_distance_expansion(rr_vec.norm(dim=-1)))
-        aa_ea = self.atom_edge_embedding(self.lig_distance_expansion(aa_vec.norm(dim=-1)))
-        ar_ea = self.ar_edge_embedding(self.rec_distance_expansion(ar_vec.norm(dim=-1)))
-        r_node, a_node = self.rec_node_embedding(rec.x), self.atom_node_embedding(atom.x)
-        if len(self.rec_emb_layers):
+        tiles = self._receptor_tiles(data, B, rr_ei, aa_ei, ar_ei)
+        if tiles is None:
+            xr, xa, rr_u, aa_u, ar_u, vecs = rec.x, atom.x, rr_ei, aa_ei, ar_ei, (rr_vec, aa_vec, ar_vec)
+        else:
+            rt, at, lt = tiles['rec'], tiles['atom'], tiles['ar']
+            xr, xa = rec.x[rt['nodes']], atom.x[at['nodes']]
+            rr_u, aa_u, ar_u = rt['edge_index'], at['edge_index'], lt['edge_index']
+            vecs = (rr_vec[rt['edges']], aa_vec[at['edges']], ar_vec[lt['edges']])
+        rr_vec_u, aa_vec_u, ar_vec_u = vecs
+        nr_u, na_u = xr.shape[0], xa.shape[0]
+        rr_ea = self.rec_edge_embedding(self.rec_distance_expansion(rr_vec_u.norm(dim=-1)))
+        aa_ea = self.atom_edge_embedding(self.lig_distance_expansion(aa_vec_u.norm(dim=-1)))
+        ar_ea = self.ar_edge_embedding(self.rec_distance_expansion(ar_vec_u.norm(dim=-1)))
+        r_node, a_node = self.rec_node_embedding(xr), self.atom_node_embedding(xa)
+        # layer-0 messages of the static groups can be shared by the copies (_shared_static_messages)
+        shareable = tiles is not None and nr_u + na_u < n_rec + n_atom and self.differentiate_convolutions \
+            and len(self.conv_layers) > 1
+        u_groups = None
+        if len(self.rec_emb_layers) or shareable:
             # joint numbering [residues | atoms] (:301-311): residue<-residue, atom<-residue, atom<-atom, residue<-atom
+            n = nr_u + na_u
+            u_groups = [self._csr(rr_u[0], rr_u[1], n, rr_ea, rr_vec_u),
+                        self._csr(ar_u[0] + nr_u, ar_u[1], n, ar_ea, ar_vec_u),
+                        self._csr(aa_u[0] + nr_u, aa_u[1] + nr_u, n, aa_ea, aa_vec_u),
+                        self._csr(ar_u[1], ar_u[0] + nr_u, n, ar_ea, ar_vec_u)]       # reversed: forward harmonics
+        if len(self.rec_emb_layers):
             node = torch.cat([r_node, a_node], 0)
-            n = n_rec + n_atom
-            groups = [self._csr(rr_ei[0], rr_ei[1], n, rr_ea, rr_vec) + (None,),
-                      self._csr(ar_ei[0] + n_rec, ar_ei[1], n, ar_ea, ar_vec) + (None,),
-                      self._csr(aa_ei[0] + n_rec, aa_ei[1] + n_rec, n, aa_ea, aa_vec) + (None,),
-                      self._csr(ar_ei[1], ar_ei[0] + n_rec, n, ar_ea, ar_vec) + (None,)]      # reversed: forward harmonics
             for layer in self.rec_emb_layers:
-                node = layer.forward_groups(node, groups, gather_scalars=ns)
-            r_node, a_node = node[:n_rec], node[n_rec:]
+                node = layer.forward_groups(node, [g + (None,) for g in u_groups], gather_scalars=ns)
+            r_node, a_node = node[:nr_u], node[nr_u:]
+        if tiles is not None:
+            r_node, a_node = r_node[rt['node_map']], a_node[at['node_map']]
+            rr_ea, aa_ea, ar_ea = rr_ea[rt['edge_map']], aa_ea[at['edge_map']], ar_ea[lt['edge_map']]
         rec.rec_node_attr, rr.rec_edge_attr, rr.edge_sh, rr.edge_weight = r_node, rr_ea, None, 1.0
         atom.atom_node_attr, aa.atom_edge_attr, aa.edge_sh, aa.edge_weight = a_node, aa_ea, None, 1.0
         ar.edge_attr, ar.edge_sh, ar.edge_weight = ar_ea, None, 1
@@ -150,6 +183,12 @@ class AAModel(CGModel):
         c['cap_la'] = int((lig_cnt.long() * atom_cnt.long()).sum())      # every ligand atom x every atom of its complex
         c['atom_batch32'] = _i32(atom.batch)
         c['gid32'] = {k: _i32(c[k][4]) for k in ('rr', 'ra', 'aa', 'ar')}
+        if shareable:
+            # the four static groups of the distinct receptors with their layer-0 group index in the nine-group list
+            # (forward_groups order: ll, lr, la, rr, rl, ra, aa, al, ar) and a zero sigma row per edge
+            zero = lambda g: torch.zeros(g[0].shape[0], dtype=torch.int32, device=rp.device)
+            c['shared_static'] = (rt['nodes'], at['nodes'], rt['node_map'], at['node_map'],
+                                  [(k, g, zero(g)) for k, g in zip((3, 8, 6, 5), u_groups) if g[0].shape[0]])
         rr._b200aa = c
         return c
 
@@ -182,8 +221,36 @@ class AAModel(CGModel):
         node = torch.cat([lig_node, rec_node, atom_node], 0)
         stat = lambda k: (c[k][0], c[k][1], c[k][2], c[k][3], None, dict(ea_add=sig, ea_add_idx=c['gid32'][k]))
         groups = [g_ll, g_lr, g_la, stat('rr'), g_rl, stat('ra'), stat('aa'), g_al, stat('ar')]
-        node = self._interaction_layers(node, groups, 3)
+        shared = self._shared_static_messages(data, c, node, sig, o_r, o_a)
+        node = self._interaction_layers(node, groups, 3, shared=(shared, (3, 5, 6, 8)) if shared is not None else None)
         return self._heads(data, c, node[:n_lig], tr_sigma, rot_sigma, tor_sigma, sync_free=True)
+
+    def _shared_static_messages(self, data, c, node, sig, o_r, o_a):
+        """Layer-0 messages of the four static groups (residue<-residue, residue<-atom, atom<-atom, atom<-residue) when the
+        batch holds copies of the same receptors at ONE diffusion time (``data._uniform_t``, the sampler's promise): their
+        node features (static embedding + sigma embedding) and edge attributes are then the same in every copy, so they
+        are accumulated once over the distinct receptors and added to every copy's rows (CGModel._shared_receptor_messages
+        does the same for the residue graph).  ``node``: the joint features [ligand | residues | atoms] entering layer 0.
+        None when there is nothing to share."""
+        if 'shared_static' not in c or not getattr(data, '_uniform_t', False):
+            return None
+        rows_r, rows_a, map_r, map_a, u_groups = c['shared_static']
+        layer = self.conv_layers[0]
+        x0 = torch.cat([node[o_r + rows_r], node[o_a + rows_a]], 0)
+        n_u, nr_u = x0.shape[0], rows_r.shape[0]
+        acc = (torch.zeros((n_u, layer.out_size), dtype=torch.float32, device=x0.device),
+               torch.zeros((n_u,), dtype=torch.float32, device=x0.device))
+        s0 = sig[:1].contiguous()
+        for k, g, zero in u_groups:
+            acc = layer.accumulate_group(x0, g + (None, dict(ea_add=s0, ea_add_idx=zero)), k, n_u, gather_scalars=self.ns,
+                                         init=acc)
+        sum_buf = torch.zeros((node.shape[0], layer.out_size), dtype=torch.float32, device=x0.device)
+        cnt_buf = torch.zeros((node.shape[0],), dtype=torch.float32, device=x0.device)
+        sum_buf[o_r:o_a].add_(acc[0][:nr_u][map_r])
+        sum_buf[o_a:].add_(acc[0][nr_u:][map_a])
+        cnt_buf[o_r:o_a].add_(acc[1][:nr_u][map_r])
+        cnt_buf[o_a:].add_(acc[1][nr_u:][map_a])
+        return sum_buf, cnt_buf
 
     def _forward_host_sized(self, data, c):
         """Forward with exactly-sized neighbour lists (the sizes are read back to the host)."""

@@ -50,34 +50,67 @@ def _rr_joint(c, n_lig):
     return c['rr_tgt32'][n_lig]
 
 
+def _block_maps(spans, dev):
+    """``spans`` = [(batch offset, rows per copy, copies, distinct id)] in batch order, the copies of a span back to back:
+    ``(rows, row_map, offsets)`` - the batch rows of copy 0 of each distinct id's first span, concatenated in order of first
+    appearance; the distinct row of every batch row; the distinct offset of each id."""
+    ar = lambda a, b: torch.arange(a, b, device=dev)
+    rows, uoff, n_u = [], {}, 0
+    for off, n1, _, uid in spans:
+        if uid not in uoff:
+            uoff[uid] = n_u
+            rows.append(ar(off, off + n1))
+            n_u += n1
+    row_map = torch.cat([(uoff[uid] + ar(0, n1)).repeat(cp) for _, n1, cp, uid in spans])
+    return torch.cat(rows), row_map, uoff
+
+
 def receptor_tiles(rec, B, ei):
     """Index maps between a batch whose receptor store carries a block layout (``hetero.receptor_blocks``) and its distinct
     receptors, numbered by concatenating copy 0 of each one's first block; None without a layout.  ``nodes`` / ``edges``:
     batch rows of those copies; ``edge_index``: their contact edges in the distinct numbering; ``node_map`` [n_rec] /
     ``edge_map`` [E]: the distinct row of every batch node / edge; ``sorted_rows`` / ``sorted_shift``: the rows of the copies
     in the contact graph sorted stably by target (targets of a copy sort together, copies in batch order) and what turns
-    their batch node numbers into distinct ones."""
+    their batch node numbers into distinct ones.  Works for any receptor-side node store with its own edges (residues and
+    their contact graph, receptor atoms and the ('atom', 'atom') edges)."""
     blocks = receptor_blocks(rec, B, ei.shape[1])
     if blocks is None:
         return None
     dev = ei.device
-    ar = lambda a, b: torch.arange(a, b, device=dev)
-    first, nodes, edges, shift, uoff, ueoff = {}, [], [], [], {}, {}
-    n_u = e_u = 0
-    for noff, eoff, n1, e1, cp, uid in blocks:
-        if uid in first:
-            continue
-        first[uid] = True
-        uoff[uid], ueoff[uid] = n_u, e_u
-        nodes.append(ar(noff, noff + n1))
-        edges.append(ar(eoff, eoff + e1))
-        shift.append(torch.full((e1,), noff - n_u, dtype=torch.long, device=dev))
-        n_u, e_u = n_u + n1, e_u + e1
-    nodes, edges, shift = torch.cat(nodes), torch.cat(edges), torch.cat(shift)
-    node_map = torch.cat([(uoff[uid] + ar(0, n1)).repeat(cp) for _, _, n1, _, cp, uid in blocks])
-    edge_map = torch.cat([(ueoff[uid] + ar(0, e1)).repeat(cp) for _, _, _, e1, cp, uid in blocks])
+    nodes, node_map, uoff = _block_maps([(noff, n1, cp, uid) for noff, _, n1, _, cp, uid in blocks], dev)
+    edges, edge_map, _ = _block_maps([(eoff, e1, cp, uid) for _, eoff, _, e1, cp, uid in blocks], dev)
+    seen, shift = set(), []
+    for noff, _, _, e1, _, uid in blocks:
+        if uid not in seen:
+            seen.add(uid)
+            shift.append(torch.full((e1,), noff - uoff[uid], dtype=torch.long, device=dev))
+    shift = torch.cat(shift)
     return dict(nodes=nodes, edges=edges, edge_index=ei[:, edges] - shift, node_map=node_map, edge_map=edge_map,
                 sorted_rows=edges, sorted_shift=shift)
+
+
+def linked_edge_tiles(src, src_tiles, dst_tiles, ei, B):
+    """Index maps of the edges between two tiled receptor-side stores (the ('atom', 'receptor') edges of all-atom graphs:
+    row 0 an atom, row 1 its residue), which the block layout does not describe by itself: the batch collates them copy by
+    copy in the order of the ``src`` store's blocks, so the edges of a copy are those whose row-0 node lies in it.
+    ``(edges, edge_index, edge_map)`` - batch rows of copy 0 of each distinct receptor, those edges in the two stores'
+    distinct numberings, the distinct row of every batch edge - or None when the batch's edges do not follow that layout.
+    Two host reads (the per-graph edge counts, the check)."""
+    blocks = receptor_blocks(src, B, src_tiles['edge_map'].shape[0])
+    cnt = torch.bincount(src.batch[ei[0]], minlength=B).tolist() if ei.shape[1] else [0] * B
+    spans, g, eoff, per_uid = [], 0, 0, {}
+    for _, _, _, _, cp, uid in blocks:
+        e1 = cnt[g]
+        if any(c != e1 for c in cnt[g:g + cp]) or per_uid.setdefault(uid, e1) != e1:
+            return None
+        spans.append((eoff, e1, cp, uid))
+        g, eoff = g + cp, eoff + e1 * cp
+    edges, edge_map, _ = _block_maps(spans, ei.device)
+    ends = torch.stack([src_tiles['node_map'][ei[0]], dst_tiles['node_map'][ei[1]]])    # every batch edge, distinct ends
+    edge_index = ends[:, edges]
+    if not torch.equal(edge_index[:, edge_map], ends):                  # each edge is the same edge of its copy 0
+        return None
+    return dict(edges=edges, edge_map=edge_map, edge_index=edge_index)
 
 
 class CGModel(nn.Module):
@@ -360,8 +393,8 @@ class CGModel(nn.Module):
         """The interaction layers over the joint graph; the last one only takes the first ``n_last`` groups, the edges that
         end on ligand atoms (models/cg_model.py:347-349).  ``merge``: one radial MLP for all edge types runs them as a
         single group (exactly-sized lists only).  ``shared = (accumulators, k)``: layer 0 starts from messages computed
-        elsewhere instead of running group ``k``.  ``per_layer = (k, [group | None per layer])``: layer l runs the given
-        group in place of group ``k`` where one is given."""
+        elsewhere instead of running group ``k`` (an int, or a tuple of group indices).  ``per_layer = (k, [group | None per
+        layer])``: layer l runs the given group in place of group ``k`` where one is given."""
         L = len(self.conv_layers)
         for l, layer in enumerate(self.conv_layers):
             use, init = (groups if l < L - 1 else groups[:n_last]), None
@@ -370,7 +403,8 @@ class CGModel(nn.Module):
                 use = use[:k] + [per_layer[1][l]] + use[k + 1:]
             if l == 0 and shared is not None:
                 init, skip = shared
-                use = use[:skip] + [None] + use[skip + 1:]
+                skip = (skip,) if isinstance(skip, int) else skip
+                use = [None if k in skip else g for k, g in enumerate(use)]
             if merge:
                 use = [tuple(torch.cat([g[k] for g in use]) if use[0][k] is not None else None for k in range(5))]
             node = layer.forward_groups(node, use, gather_scalars=self.ns, init=init)

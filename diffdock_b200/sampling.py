@@ -588,10 +588,19 @@ def sampling(data_list, model, inference_steps, tr_schedule, rot_schedule, tor_s
     return data_list, confidence
 
 
+def pack_cost(poses, all_atoms=False):
+    """The cost of one complex in a pack: poses x ligand atoms x receptor nodes, the capacity of its ligand <- receptor
+    cross graphs that sets a step's memory.  Receptor nodes are the residues, plus the receptor atoms for an all-atom score
+    model (``all_atoms``; its ligand <- atom graph is the larger of the two)."""
+    g = poses[0]
+    n_rec = int(g['receptor'].num_nodes) + (int(g._nodes['atom'].num_nodes) if all_atoms else 0)
+    return len(poses) * int(g['ligand'].num_nodes) * n_rec
+
+
 def pack_plan(costs, max_pairs):
-    """Greedy packing of complexes, in the given order, into batches whose summed cost (poses x ligand atoms x residues, the
-    cross-graph capacity that sets a step's memory) stays within ``max_pairs``; a complex larger than the budget gets a
-    batch of its own.  Returns lists of complex indices."""
+    """Greedy packing of complexes, in the given order, into batches whose summed cost (``pack_cost``: poses x ligand atoms x
+    receptor nodes, the cross-graph capacity that sets a step's memory) stays within ``max_pairs``; a complex larger than
+    the budget gets a batch of its own.  Returns lists of complex indices."""
     packs, cur, total = [], [], 0
     for i, cost in enumerate(costs):
         if cur and total + cost > max_pairs:
@@ -614,12 +623,16 @@ def sample_packed(complexes, model, inference_steps, tr_schedule, rot_schedule, 
                   confidence_model_args=None, max_pairs=None, cuda_graph=None, noise_fn=None, visualization_list=None,
                   t_schedule=None):
     """Several docking jobs in one reverse-diffusion step.  ``complexes``: a list of pose lists, each what ``sampling`` takes
-    as ``data_list`` for one complex (``HeteroGraph`` items).  The complexes are packed greedily, in order, into batches of
-    at most ``max_pairs`` poses x ligand atoms x residues (default ``PACK_MAX_PAIRS``; ``pack_plan``); each batch is one
+    as ``data_list`` for one complex (``HeteroGraph`` items; all-atom graphs for an ``AAModel``).  The complexes are packed
+    greedily, in order, into batches of at most ``max_pairs`` poses x ligand atoms x receptor nodes (``pack_cost``: residues,
+    plus receptor atoms for an all-atom model; default ``PACK_MAX_PAIRS``; ``pack_plan``); each batch is one
     ``hetero.collate_packed`` and runs its steps as one captured CUDA graph where ``sampling`` would, else eagerly, with
     the packed pose update (ddb200_pose_update_packed) and a per-complex NaN guard.  Noise is always Philox, keyed by
     ``(complex_ids[k] << 32) | pose`` (``complex_ids`` default 0 .. K-1).  ``confidence_data``: one list of confidence graphs
     per complex, ranked complex by complex with ``sampling``'s code.
+
+    Score models: ``CGModel``, ``CGOldModel`` and ``AAModel``; an all-atom model without per-step cropping
+    (``model_args.crop_beyond``), which is not built for receptor atoms.
 
     Returns ``[(data_list, confidence)]`` per complex, in input order: what ``sampling(poses, ..., rng='philox',
     pose_keys=keys, batch_size >= len(poses))`` returns for each complex, up to the summation order of atomics.  The
@@ -629,9 +642,13 @@ def sample_packed(complexes, model, inference_steps, tr_schedule, rot_schedule, 
                                   "t_schedule are sampling() options")
     from .aa_model import AAModel
     from .old_aa_model import AAOldModel
-    if getattr(model_args, 'all_atoms', False) or isinstance(model, (AAModel, AAOldModel)):
-        raise NotImplementedError("sample_packed runs the coarse-grained score models (CGModel, CGOldModel); all-atom score "
-                                  "models are sampled one complex per sampling() call")
+    all_atoms = isinstance(model, AAModel)
+    if isinstance(model, AAOldModel) or (getattr(model_args, 'all_atoms', False) and not all_atoms):
+        raise NotImplementedError("sample_packed runs the score models CGModel, CGOldModel and AAModel; model_args.all_atoms "
+                                  "asks for an all-atom score model (AAModel)")
+    if all_atoms and getattr(model_args, 'crop_beyond', None) is not None:
+        raise NotImplementedError("sample_packed does not crop all-atom receptors per step (crop_beyond): the device-side "
+                                  "crop covers residues only; sample such complexes one per sampling() call")
     device = torch.device(device)
     if device.type != 'cuda':
         raise RuntimeError("diffdock_b200.sample_packed runs on a CUDA device only (no CPU fallback)")
@@ -641,7 +658,7 @@ def sample_packed(complexes, model, inference_steps, tr_schedule, rot_schedule, 
     complex_ids = list(range(K)) if complex_ids is None else [int(i) for i in complex_ids]
     if len(complex_ids) != K:
         raise ValueError("one complex id per complex")
-    costs = [len(p) * int(p[0]['ligand'].num_nodes) * int(p[0]['receptor'].num_nodes) for p in complexes]
+    costs = [pack_cost(p, all_atoms) for p in complexes]
     packs = pack_plan(costs, PACK_MAX_PAIRS if max_pairs is None else max_pairs)
     use_torsion = not model_args.no_torsion
     graphed = _use_cuda_graph(model, model_args, None, None, 0, 0, cuda_graph)
