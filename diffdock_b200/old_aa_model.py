@@ -15,18 +15,22 @@ Where every convolution has a fused-kernel shape and no complex has more than 10
 no device->host read after the per-batch constants (``_static``, ``_forward_sync_free``), as CGOldModel's score mode does:
 
 1. The residue and atom node embeddings are computed once per batch with the sigma embedding set to zero; each call adds
-   ``M . sigma_emb`` per complex (the encoders are affine in the sigma embedding).  A batch of B poses of one receptor
-   (``_unique`` on the residue and atom stores, diffdock_b200.hetero.collate_shared_receptor) embeds one copy.
+   ``M . sigma_emb`` per complex (the encoders are affine in the sigma embedding).  A batch whose residue and atom stores
+   carry a block layout - B poses of one receptor (``_unique``, diffdock_b200.hetero.collate_shared_receptor) or several
+   complexes (``_blocks``, diffdock_b200.hetero.collate_packed) - embeds each distinct receptor once and gathers the rows
+   onto the batch through ``node_map`` (diffdock_b200.cg_model.receptor_tiles / linked_edge_tiles).
 2. The three static edge sets (residue-residue, atom-atom, atom-residue) are CSR-sorted by target once per batch; the
    residue<-atom group is the atom<-residue list sorted by residue, reading its attributes through ``edge_perm``.  Their
-   edge attributes depend on sigma and are embedded per call (one copy's when the batch holds one receptor at one time).
+   edge attributes depend on sigma and are embedded per call: per batch edge, or - for a block layout at one time - per
+   distinct receptor edge, read by every copy through ``edge_perm``.
 3. The ligand graph and the ligand<-residue / ligand<-atom graphs go into capacity buffers with device counts; the
    atom<-ligand and residue<-ligand groups are permutations of those lists with the forward vector (``vec_sign = +1``).
 4. Nine fused launches per layer, each with its own radial MLP, into one accumulator per (target type, convolution);
    three chained ddb200_tpconv_finalize calls per target type give ``pad(x) + up + up + up`` in the reference's order.
-5. In a batch of one receptor at one time (``_uniform_t``: the sampler's ranking call at t = 0) the four layer-0 groups that
-   end on residues or atoms and start from them (residue<-residue, residue<-atom, atom<-atom, atom<-residue) see the same
-   inputs in every copy: their messages are computed for copy 0 and added to every copy.
+5. In a batch of repeated receptors at one time (``_uniform_t``: the sampler's ranking call at t = 0) the four layer-0
+   groups that end on residues or atoms and start from them (residue<-residue, residue<-atom, atom<-atom, atom<-residue)
+   see the same inputs in every copy: their messages are computed over the distinct receptors' edges and gathered onto
+   every copy's rows.
 
 CUDA only, inference only.  No CPU fallback.
 """
@@ -40,7 +44,9 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
+from .aa_model import AAModel
 from .cg_model import CGModel, _flat, _i32
+from .hetero import receptor_blocks
 from .irreps import irreps_str, sh_irreps
 from .layers import (GaussianSmearing, OldAtomEncoder, _mlp, check_confidence_widths, check_forward, confidence_head,
                      cross_cutoff, cross_graph, edge_weight, ligand_graph)
@@ -55,9 +61,9 @@ _LIG_SUM, _REC_SUM, _ATOM_SUM = (0, 2, 1), (6, 8, 7), (3, 4, 5)
 
 
 def _uniq(st, B, n_edges):
-    """True when ``st`` carries ``_unique = (nodes, edges, copies)`` for this batch of B copies."""
-    u = getattr(st, '_unique', None)
-    return u is not None and u[2] == B and u[0] * B == st.pos.shape[0] and u[1] * B == n_edges
+    """True when ``st`` carries ``_unique = (nodes, edges, copies)`` for this batch of B copies: the one-block case of
+    ``hetero.receptor_blocks``, which the forward reads for every block layout."""
+    return getattr(st, '_unique', None) is not None and receptor_blocks(st, B, n_edges) is not None
 
 
 def _csr(tgt, n_rows):
@@ -75,6 +81,7 @@ class AAOldModel(nn.Module):
     _cross_graph_sync_free = CGModel._cross_graph_sync_free
     _cross_edge_embedding = CGModel._cross_edge_embedding
     _edge_embed_in_kernel = CGModel._edge_embed_in_kernel
+    _receptor_tiles = staticmethod(AAModel._receptor_tiles)      # the all-atom block layout's index maps
     _bn = staticmethod(CGOldModel._bn)
 
     def __init__(self, t_to_sigma, device, timestep_emb_func, in_lig_edge_features=4, sigma_embed_dim=32, sh_lmax=2,
@@ -178,9 +185,11 @@ class AAOldModel(nn.Module):
     def _static(self, data):
         """Per-batch constants, cached on ``data`` (host reads of the node counts): the sigma-free residue and atom node
         embeddings with their sigma maps, the static edge sets CSR-sorted by target in the joint numbering
-        [ligand | residues | atoms] with the complex of each edge, copy 0 of them in the local numbering
-        [residues | atoms] of one copy when the batch holds ``copies`` identical receptors, and the ligand / cross-graph
-        constants of CGModel._static_sync_free."""
+        [ligand | residues | atoms] with the complex of each edge, and the ligand / cross-graph constants of
+        CGModel._static_sync_free.  A batch whose residue and atom stores carry a block layout (``AAModel._receptor_tiles``:
+        ``collate_shared_receptor``'s one receptor, ``collate_packed``'s distinct receptors) also gets the distinct
+        receptors' edge vectors with the distinct row of every sorted edge (``perm``), and - when some receptor is
+        repeated - their four static groups in the local numbering [distinct residues | distinct atoms] (``shared``)."""
         rec, atom, lig = data['receptor'], data['atom'], data['ligand']
         rr, aa, ar, ll = data['receptor', 'receptor'], data['atom', 'atom'], data['atom', 'receptor'], data['ligand', 'ligand']
         hit = getattr(rr, '_b200_v10aa', None)
@@ -191,44 +200,49 @@ class AAOldModel(nn.Module):
         o_r, o_a = n_lig, n_lig + n_rec
         N = o_a + n_atom
         rr_ei, aa_ei, ar_ei = rr.edge_index.long(), aa.edge_index.long(), ar.edge_index.long()
-        copies = B if B > 1 and _uniq(rec, B, rr_ei.shape[1]) and _uniq(atom, B, aa_ei.shape[1]) \
-            and ar_ei.shape[1] % B == 0 else 1
-        n1r, n1a = n_rec // copies, n_atom // copies
-        c = {'copies': copies, 'n1': (n1r, n1a)}
-        # node embeddings with the sigma embedding set to zero (:401, :424), one copy, the LM layer included
-        for key, st, enc, n1 in (('rec', rec, self.rec_node_embedding, n1r), ('atom', atom, self.atom_node_embedding, n1a)):
-            x1 = st.x[:n1].float()
-            base = enc(torch.cat([x1, x1.new_zeros((n1, S))], 1))
-            c[key + '_base'] = base.repeat(copies, 1) if copies > 1 else base
+        tiles = self._receptor_tiles(data, B, rr_ei, aa_ei, ar_ei)
+        rt, at, lt = (tiles['rec'], tiles['atom'], tiles['ar']) if tiles is not None else (None, None, None)
+        c = {}
+        # node embeddings with the sigma embedding set to zero (:401, :424), once per distinct receptor, the LM layer included
+        for key, st, enc, t in (('rec', rec, self.rec_node_embedding, rt), ('atom', atom, self.atom_node_embedding, at)):
+            x1 = (st.x[t['nodes']] if t is not None else st.x).float()
+            base = enc(torch.cat([x1, x1.new_zeros((x1.shape[0], S))], 1))
+            c[key + '_base'] = base[t['node_map']] if t is not None else base
             c[key + '_sigma_map'] = sigma_map(enc, S, st.x.shape[1])
         c['rec_gid'], c['atom_gid'] = rec.batch, atom.batch
         # static edge sets (:404-445, :486): row 0 = convolution target, vector gathered - target, sigma of the target's complex
         rp, ap = rec.pos.float(), atom.pos.float()
-        spec = {'rr': (rr_ei[0] + o_r, rr_ei[1] + o_r, rp[rr_ei[1]] - rp[rr_ei[0]], rec.batch[rr_ei[0]], self.rec_max_radius),
-                'aa': (aa_ei[0] + o_a, aa_ei[1] + o_a, ap[aa_ei[1]] - ap[aa_ei[0]], atom.batch[aa_ei[0]], self.lig_max_radius),
-                'ar': (ar_ei[0] + o_a, ar_ei[1] + o_r, rp[ar_ei[1]] - ap[ar_ei[0]], atom.batch[ar_ei[0]], None)}
-        for k, (tgt, src, vec, gid, max_r) in spec.items():
+        spec = {'rr': (rr_ei[0] + o_r, rr_ei[1] + o_r, rp[rr_ei[1]] - rp[rr_ei[0]], rec.batch[rr_ei[0]], self.rec_max_radius, rt),
+                'aa': (aa_ei[0] + o_a, aa_ei[1] + o_a, ap[aa_ei[1]] - ap[aa_ei[0]], atom.batch[aa_ei[0]], self.lig_max_radius, at),
+                'ar': (ar_ei[0] + o_a, ar_ei[1] + o_r, rp[ar_ei[1]] - ap[ar_ei[0]], atom.batch[ar_ei[0]], None, lt)}
+        ew = lambda vec, max_r: _flat(self.get_edge_weight(vec, max_r)) if max_r is not None else None
+        for k, (tgt, src, vec, gid, max_r, t) in spec.items():
             t32, order = _csr(tgt, N)
-            vec = vec[order].contiguous()
-            c[k] = dict(tgt=t32, src=_i32(src[order]), vec=vec, gid=_i32(gid[order]),
-                        ew=_flat(self.get_edge_weight(vec, max_r)) if max_r is not None else None)
+            vs = vec[order].contiguous()
+            c[k] = dict(tgt=t32, src=_i32(src[order]), vec=vs, gid=_i32(gid[order]), ew=ew(vs, max_r))
+            if t is not None:       # the distinct receptors' edges, and the distinct row of every sorted edge
+                vu = vec[t['edges']].contiguous()
+                c[k].update(perm=_i32(t['edge_map'][order]), vec_u=vu, ew_u=ew(vu, max_r),
+                            row_u=torch.zeros(vu.shape[0], dtype=torch.int32, device=vu.device))
         # residue <- atom (:264-266): the atom <- residue edges sorted by residue, forward attributes and vector
         t32, order = _csr(c['ar']['src'].long(), N)
         c['ra'] = dict(tgt=t32, src=c['ar']['tgt'][order].contiguous(), perm=_i32(order))
-        if copies > 1:
-            # copy 0 of every sorted list comes first (its targets sort first); the other copies read its attributes
-            local = {'rr': (o_r, 0, o_r, 0), 'aa': (o_a, n1r, o_a, n1r), 'ar': (o_a, n1r, o_r, 0)}
-            for k, (to, tb, so, sb) in local.items():
-                d, E = c[k], c[k]['tgt'].shape[0]
-                e1 = E // copies
-                d['perm'] = _i32(torch.arange(E, device=rp.device) % max(e1, 1))
-                c[k + '0'] = dict(tgt=_i32(d['tgt'][:e1] - to + tb), src=_i32(d['src'][:e1] - so + sb),
-                                  vec=d['vec'][:e1].contiguous(), row=torch.zeros(e1, dtype=torch.int32, device=rp.device),
-                                  ew=d['ew'][:e1].contiguous() if d['ew'] is not None else None)
-            e1 = c['ra']['tgt'].shape[0] // copies
-            c['ra']['perm_shared'] = _i32(c['ra']['perm'] % max(e1, 1))
-            c['ra0'] = dict(tgt=_i32(c['ra']['tgt'][:e1] - o_r), src=_i32(c['ra']['src'][:e1] - o_a + n1r),
-                            perm=c['ra']['perm'][:e1].contiguous())
+        if tiles is not None:
+            c['ra']['perm_u'] = c['ar']['perm'][order].contiguous()
+            nr_u, na_u = rt['nodes'].shape[0], at['nodes'].shape[0]
+            if nr_u + na_u < n_rec + n_atom and self.num_conv_layers > 1:
+                # the four layer-0 groups between residues and atoms over the distinct receptors, numbered [residues |
+                # atoms]; each reads the attributes of its distinct edge (the atom-residue edges' for residue <- atom)
+                n_u = nr_u + na_u
+                loc = {'rr': (rt['edge_index'][0], rt['edge_index'][1]),
+                       'aa': (at['edge_index'][0] + nr_u, at['edge_index'][1] + nr_u),
+                       'ar': (lt['edge_index'][0] + nr_u, lt['edge_index'][1]),
+                       'ra': (lt['edge_index'][1], lt['edge_index'][0] + nr_u)}
+                groups = {}
+                for k, (tgt, src) in loc.items():
+                    t32, order = _csr(tgt, n_u)
+                    groups[k] = (t32, _i32(src[order]), _i32(order))
+                c['shared'] = (rt['nodes'], at['nodes'], rt['node_map'], at['node_map'], groups)
         # ligand graph and cross-graph constants (CGModel._static_sync_free) and the atom side of the ligand<-atom graph
         c['rec_ptr'], c['atom_ptr'], c['lig_ptr'] = (ops.segment_ptr(s.batch, B) for s in (rec, atom, lig))
         c['rr_tgt_batch'] = rec.batch[rr_ei[0]]
@@ -256,7 +270,8 @@ class AAOldModel(nn.Module):
         ns, n_lig = self.ns, lig.batch.shape[0]
         o_r, o_a = n_lig, n_lig + rec.pos.shape[0]
         N = o_a + atom.pos.shape[0]
-        shared = c['copies'] > 1 and getattr(data, '_uniform_t', False)     # one receptor at one time
+        # distinct receptors at one time: every copy's static edge attributes and layer-0 messages are its distinct one's
+        uniform = 'perm_u' in c['ra'] and getattr(data, '_uniform_t', False)
         tr_sigma = data.complex_t['tr']                                      # confidence mode: the times are the sigmas
         sig = self.timestep_emb_func(tr_sigma)                               # [B, S], per complex
 
@@ -266,22 +281,19 @@ class AAOldModel(nn.Module):
         emb = {'rr': (self.rec_edge_embedding, self.rec_distance_expansion),
                'aa': (self.atom_edge_embedding, self.lig_distance_expansion),
                'ar': (self.ar_edge_embedding, self.rec_distance_expansion)}
-        g, g0 = {}, {}
+        g = {}
         for k, (mlp, gs) in emb.items():
             d = c[k]
-            if shared:      # one copy's attributes; the copies read them through edge_perm
-                d0 = c[k + '0']
-                ea = self._static_edge_attr(sig[:1], d0['vec'], d0['row'], mlp, gs)
-                g[k] = (d['tgt'], d['src'], ea, d0['vec'], d0['ew'], dict(edge_perm=d['perm']))
-                g0[k] = (d0['tgt'], d0['src'], ea, d0['vec'], d0['ew'], {})
+            if uniform:     # the distinct receptors' attributes; every edge reads its distinct row through edge_perm
+                ea = self._static_edge_attr(sig[:1], d['vec_u'], d['row_u'], mlp, gs)
+                g[k] = (d['tgt'], d['src'], ea, d['vec_u'], d['ew_u'], dict(edge_perm=d['perm']))
             else:
                 ea = self._static_edge_attr(sig, d['vec'], d['gid'], mlp, gs)
                 g[k] = (d['tgt'], d['src'], ea, d['vec'], d['ew'], {})
         ra = c['ra']
         g['ra'] = (ra['tgt'], ra['src'], g['ar'][2], g['ar'][3], None,
-                   dict(edge_perm=ra['perm_shared'] if shared else ra['perm']))
-        if shared:
-            g0['ra'] = (c['ra0']['tgt'], c['ra0']['src'], g0['ar'][2], g0['ar'][3], None, dict(edge_perm=c['ra0']['perm']))
+                   dict(edge_perm=ra['perm_u'] if uniform else ra['perm']))
+        shared = uniform and 'shared' in c
 
         # -- ligand graph (:358-398) and ligand cross graphs (:447-485) --------------------------------------------------
         g_ll = self._ligand_edges_sync_free(data, c)
@@ -304,7 +316,7 @@ class AAOldModel(nn.Module):
             last = l == L - 1
             convs = C[9 * l:9 * l + 9]
             ks = (0, 1, 2) if last else range(9)
-            acc = self._shared_static_messages(x, c, g0, o_r, o_a, N, convs) if (l == 0 and shared and not last) else {}
+            acc = self._shared_static_messages(x, c, g, o_r, o_a, N, convs) if (l == 0 and shared and not last) else {}
             for k in ks:        # raw sums per convolution; rows of a sum: its target type's rows in the joint numbering
                 if k not in acc:
                     acc[k] = convs[k].accumulate_group(x, groups[k][0], 0, groups[k][1], ns)
@@ -319,23 +331,28 @@ class AAOldModel(nn.Module):
             x = out
         return x
 
-    def _shared_static_messages(self, x, c, g0, o_r, o_a, N, convs):
+    def _shared_static_messages(self, x, c, g, o_r, o_a, N, convs):
         """Layer-0 sums of the four groups between residues and atoms (residue<-residue, residue<-atom, atom<-atom,
-        atom<-residue) for a batch of B poses of ONE receptor at ONE time: their node features and edge attributes are the
-        same in every copy, so the sums are computed for copy 0 (local numbering [residues | atoms] of one copy) and
-        added to every copy's rows."""
-        B, (n1r, n1a) = c['copies'], c['n1']
-        x0 = torch.cat([x[o_r:o_r + n1r], x[o_a:o_a + n1a]], 0)
+        atom<-residue) for a batch of copies of the same receptors at ONE time: their node features and edge attributes are
+        the same in every copy, so the sums are computed once over the distinct receptors (local numbering [distinct
+        residues | distinct atoms], ``c['shared']``) and gathered onto every copy's rows through the node maps.  ``g``:
+        the batch's static groups, whose attribute arrays are already the distinct edges'."""
+        rows_r, rows_a, map_r, map_a, local = c['shared']
+        nr_u = rows_r.shape[0]
+        x0 = torch.cat([x[o_r + rows_r], x[o_a + rows_a]], 0)
+        n_u = x0.shape[0]
         D = convs[0].out_size
         acc = {}
-        for k, key, lo, n_full in ((6, 'rr', o_r, o_a), (8, 'ra', o_r, o_a), (3, 'aa', o_a, N), (5, 'ar', o_a, N)):
-            to_atom = lo == o_a
-            n_loc, m = (n1r + n1a, n1a) if to_atom else (n1r, n1r)
-            s0, n0 = convs[k].accumulate_group(x0, g0[key], 0, n_loc, self.ns)
-            s = torch.zeros((n_full, D), device=x.device)
-            n = torch.zeros((n_full,), device=x.device)
-            s[lo:].view(B, m, D).add_(s0[n_loc - m:].unsqueeze(0))
-            n[lo:].view(B, m).add_(n0[n_loc - m:].unsqueeze(0))
+        for k, key, lo, hi, part, node_map in ((6, 'rr', o_r, o_a, slice(0, nr_u), map_r),
+                                               (8, 'ra', o_r, o_a, slice(0, nr_u), map_r),
+                                               (3, 'aa', o_a, N, slice(nr_u, n_u), map_a),
+                                               (5, 'ar', o_a, N, slice(nr_u, n_u), map_a)):
+            tgt, src, perm = local[key]
+            s0, n0 = convs[k].accumulate_group(x0, (tgt, src, *g[key][2:5], dict(edge_perm=perm)), 0, n_u, self.ns)
+            s = torch.zeros((hi, D), device=x.device)
+            n = torch.zeros((hi,), device=x.device)
+            s[lo:] = s0[part][node_map]
+            n[lo:] = n0[part][node_map]
             acc[k] = (s, n)
         return acc
 
