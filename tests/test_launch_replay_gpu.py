@@ -132,8 +132,11 @@ class Recorder:
     def __init__(self, mp, conf_model=None):
         from diffdock_b200 import _lib
         from diffdock_b200.tensor_layers import TensorProductConvLayer
-        self.records, self.plans, self.depth, self.active = [], {}, 0, False
+        # records of eager launches, and of launches made while a CUDA graph was being captured: the clones of the latter
+        # are part of the graph, so every replay refreshes them with that replay's values
+        self.records, self.captured, self.plans, self.depth, self.active = [], [], {}, 0, False
         self.matched, self.escaped = Counter(), Counter()
+        self.cap_matched, self.cap_escaped = Counter(), Counter()       # the same counts, of calls made during a capture
         self.radial_ctx, self.conf_model, self.call_mutation = None, conf_model, {}
         for path in sorted({p for ps in WRAPPED.values() for p in ps}):
             mod, name = _resolve(path)
@@ -166,6 +169,8 @@ class Recorder:
             key = name + ':size' if name in SIZE_QUERIES and a and a[0] is None else name
             if self.active:
                 (self.matched if self.depth else self.escaped)[key] += 1
+                if torch.cuda.is_current_stream_capturing():
+                    (self.cap_matched if self.depth else self.cap_escaped)[key] += 1
             if name in self.call_mutation:
                 a = self.call_mutation[name](a)
             return fn(*a)
@@ -194,15 +199,15 @@ class Recorder:
                     pre['slot_in_ptr'] = args['slot_in'].data_ptr() if args['slot_in'] is not None else None
                 if path in SUM_PTR:
                     pre['sum_ptr'] = args['sum_buf'].data_ptr()
-                self.records.append((path, pre, _clone(ret), post, self.radial_ctx))
+                entry = (path, pre, _clone(ret), post, self.radial_ctx)
+                (self.captured if torch.cuda.is_current_stream_capturing() else self.records).append(entry)
             return ret
         return g
 
     def start(self):
         torch.cuda.synchronize()
-        self.records.clear()
-        self.matched.clear()
-        self.escaped.clear()
+        for c in (self.records, self.captured, self.matched, self.escaped, self.cap_matched, self.cap_escaped):
+            c.clear()
         self.active = True
 
     def stop(self):
@@ -398,7 +403,7 @@ def check_graph_fill(rec, a, ret, post, ctx):
             assert bool((perm[E:] == 0).all())
     kind = 'graph_fill'
     if a['slot_in'] is not None:          # reverse pass: perm[k] is the forward position of the same pair
-        fwd = [r for r in rec.records[:rec._cur] if r[0] == 'ops.graph_fill'
+        fwd = [r for r in rec._replaying[:rec._cur] if r[0] == 'ops.graph_fill'
                and r[3]['slot_ptr'] == a['slot_in_ptr']]
         assert fwd, "reverse pass without its forward pass"
         fa, fret = fwd[-1][1], fwd[-1][2]
@@ -525,22 +530,26 @@ CHECKS = {'fused.fused_conv': check_fused, 'ops.tpconv_accumulate': check_tpconv
           'ops.pose_update_packed': check_pose_packed}
 
 
-def replay(rec, workload):
-    """Checks every recorded launch; returns {kind: (largest error, tolerance, launches, failures)} and asserts that no
-    ddb200 call escaped the recorder."""
+def replay(rec, workload, records=None, clear=True, table=TABLE):
+    """Checks every launch of ``records`` (default: the eager records); returns {kind: (largest error, tolerance, launches,
+    failures)} and asserts that no ddb200 call escaped the recorder.  ``clear``: empty ``records`` afterwards (the captured
+    records are kept: the next replay of their graph refreshes them).  ``table``: where the largest errors are kept."""
+    records = rec.records if records is None else records
     escaped = {k: v for k, v in rec.escaped.items() if k not in EXEMPT and k.split(':')[0] not in EXEMPT}
     assert not escaped, f"{workload}: ddb200 calls outside any recorded wrapper: {escaped}"
     rec.irreps = {}
     out = {}
-    for i, (path, a, ret, post, ctx) in enumerate(rec.records):
+    rec._replaying = records
+    for i, (path, a, ret, post, ctx) in enumerate(records):
         rec._cur = i
         kind, err, tol, detail = CHECKS[path](rec, a, ret, post, ctx)
         e, t, n, bad = out.get(kind, (0.0, tol, 0, []))
         ok = err < tol if tol > 0 else err == 0.0
         out[kind] = (max(e, err), tol, n + 1, bad + ([(i, err, detail)] if not ok else []))
-    rec.records.clear()
+    if clear:
+        records.clear()
     for kind, (e, t, n, bad) in out.items():
-        cell = TABLE[(workload, kind)]
+        cell = table[(workload, kind)]
         cell[0], cell[1] = max(cell[0], e), cell[1] + n
     torch.cuda.empty_cache()
     return out
