@@ -153,6 +153,11 @@ def radius(x, y, x_ptr, y_batch, r=1.0, r_per_graph=None, max_num_neighbors=32, 
     if r_per_graph is not None:
         r_per_graph = r_per_graph.reshape(-1).float().contiguous()
     count = torch.empty(n_y, dtype=torch.int32, device=x.device)
+    if x.shape[0] == 0:
+        # nothing to search (a receptor that crop_beyond cropped to no residue): no pair, as torch_cluster.radius returns;
+        # the entry points take no null x
+        count.zero_()
+        return count.new_empty(0), count.new_empty(0), count
     L = _lib.lib()
     rc = L.ddb200_radius_count(_ptr(x), _ptr(y), _ptr(x_ptr), _ptr(yb), _ptr(r_per_graph), float(r), n_y,
                                int(max_num_neighbors), int(exclude_self), _ptr(count), _stream())
