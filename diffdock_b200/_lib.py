@@ -48,6 +48,14 @@ SIGNATURES = {
                                       _vp, _vp, _vp]),
 }
 
+# the deterministic (fixed-point) convolutions of the same library; mirrors include/diffdock_b200_fixed.h one to one
+FIXED_SIGNATURES = {
+    'ddb200_tpconv_accumulate_fixed': (_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
+    'ddb200_tpconv_finalize_fixed': (_int, [_vp, _vp, _i64, _int, _int, _vp, _vp, _vp, _i64, _int, _vp, _vp]),
+    'ddb200_fused_conv_fixed': (_int, [_vp, _vp, _vp, _vp]),      # (args, int64 sum, int32 error word, stream)
+    'ddb200_fused_conv_so_fixed': (_int, [_vp, _vp, _vp, _vp]),
+}
+
 
 def lib():
     global _lib
@@ -57,7 +65,7 @@ def lib():
                 f"{LIB_PATH} not found: build the CUDA extension first (python -c 'import __graft_entry__ as g; "
                 f"g.build()').  diffdock_b200 has no CPU fallback.")
         _lib = C.CDLL(LIB_PATH)
-        for name, (res, args) in SIGNATURES.items():
+        for name, (res, args) in (SIGNATURES | FIXED_SIGNATURES).items():
             fn = getattr(_lib, name)
             fn.restype, fn.argtypes = res, args
     return _lib

@@ -238,14 +238,12 @@ class AAModel(CGModel):
         layer = self.conv_layers[0]
         x0 = torch.cat([node[o_r + rows_r], node[o_a + rows_a]], 0)
         n_u, nr_u = x0.shape[0], rows_r.shape[0]
-        acc = (torch.zeros((n_u, layer.out_size), dtype=torch.float32, device=x0.device),
-               torch.zeros((n_u,), dtype=torch.float32, device=x0.device))
+        acc = ops.new_accumulators(n_u, layer.out_size, x0.device)
         s0 = sig[:1].contiguous()
         for k, g, zero in u_groups:
             acc = layer.accumulate_group(x0, g + (None, dict(ea_add=s0, ea_add_idx=zero)), k, n_u, gather_scalars=self.ns,
                                          init=acc)
-        sum_buf = torch.zeros((node.shape[0], layer.out_size), dtype=torch.float32, device=x0.device)
-        cnt_buf = torch.zeros((node.shape[0],), dtype=torch.float32, device=x0.device)
+        sum_buf, cnt_buf = ops.new_accumulators(node.shape[0], layer.out_size, x0.device)
         sum_buf[o_r:o_a].add_(acc[0][:nr_u][map_r])
         sum_buf[o_a:].add_(acc[0][nr_u:][map_a])
         cnt_buf[o_r:o_a].add_(acc[1][:nr_u][map_r])

@@ -632,8 +632,7 @@ class CGModel(nn.Module):
         g0 = (t0, s0, ea0, vec0, ew0, dict(ea_add=sig[:1].contiguous(), ea_add_idx=zero_idx))
         sum0, cnt0 = layer.accumulate_group(rec_node[tiles['nodes']], g0, 2, n_u, gather_scalars=self.ns)
         N = n_lig + rec_node.shape[0]
-        sum_buf = torch.zeros((N, layer.out_size), dtype=torch.float32, device=sum0.device)
-        cnt_buf = torch.zeros((N,), dtype=torch.float32, device=sum0.device)
+        sum_buf, cnt_buf = ops.new_accumulators(N, layer.out_size, sum0.device)
         sum_buf[n_lig:].add_(sum0[tiles['node_map']])
         cnt_buf[n_lig:].add_(cnt0[tiles['node_map']])
         return sum_buf, cnt_buf

@@ -32,6 +32,7 @@
 #include <stdlib.h>
 
 #include "../../include/diffdock_b200.h"
+#include "../../include/diffdock_b200_fixed.h"
 #include "sm90.cuh"
 
 namespace {
@@ -60,6 +61,19 @@ constexpr int SO_STAGES = 3, SO_MAX_PATHS = 32, SO_MTAB = 128;
 // fire-and-forget global reduction (atomicAdd here may be compiled to an atomic that returns its old value)
 __device__ __forceinline__ void red_add(float* addr, float v) {
   asm volatile("red.global.add.f32 [%0], %1;" ::"l"(addr), "f"(v) : "memory");
+}
+// 64-bit integer reduction: the fixed-point accumulators of the deterministic instantiations (two's complement, so a
+// signed sum is an unsigned one)
+__device__ __forceinline__ void red_add_u64(long long* addr, long long v) {
+  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(addr), "l"((unsigned long long)v) : "memory");
+}
+// v * 2^32 rounded to nearest (even), as a 64-bit integer.  |v| >= 2^31 and non-finite values saturate and set the sticky
+// error word *err (bit 0), which the host reads after the work is done.
+__device__ __forceinline__ long long to_fixed(float v, int* err) {
+  const float s = v * 0x1p32f;
+  if (fabsf(s) < 0x1p63f) return __float2ll_rn(s);
+  atomicOr(err, 1);
+  return v > 0.f ? 0x7fffffffffffffffLL : (v < 0.f ? -0x7fffffffffffffffLL : 0LL);
 }
 __device__ __forceinline__ void wgmma_wait_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
@@ -121,6 +135,7 @@ struct FusedParams {
   const float* x; long long ld_x; int x_vec2;        // node irreps gathered by src
   const float* vec; const float* ew; int lmax;
   float* sum; int d_out; float* cnt;
+  long long* sum_fx; int* err;                       // deterministic instantiations: int64 accumulator (2^-32 units), error word
   long long n_edges; const int* n_edges_dev;
   unsigned long long* dbg;                           // optional [32] clock counters (DDB200_FUSED_DEBUG=1), else nullptr
 };
@@ -264,7 +279,7 @@ __device__ __forceinline__ void prefetch_tile(const float* xrow, const int* ti, 
 // adds the copies, sums runs of equal targets (CSR order makes them contiguous; unsorted input just yields runs of length
 // one) and issues ONE fully coalesced RED.ADD per run for output value i.  A slice (SO: components K0 .. K0 + DOUT - 1 of a
 // DFULL-component block) lands at w DFULL + K0 + k of the block.
-template <int MULOUT, int DOUT, int DFULL = DOUT, int K0 = 0>
+template <int MULOUT, int DOUT, int DFULL = DOUT, int K0 = 0, bool FIXED = false>
 __device__ __forceinline__ void flush(const FusedParams& p, float* __restrict__ acc, float* buf, int r0, int q, int w4,
                                       int lane, int dst_s, uint32_t head_mask, int out_off, int bar) {
   using S = Slots<MULOUT>;
@@ -308,20 +323,45 @@ __device__ __forceinline__ void flush(const FusedParams& p, float* __restrict__ 
   if (32 * half < NACC) {
     const bool act = i < NACC;
     const float* col = buf + 32 * (w4 & 1) * LD + (act ? i : 0);
-    float s = 0.f;
+    if constexpr (FIXED) {
+      // deterministic: each edge's value (its copies added in a fixed order) is converted on its own and the run is
+      // summed as integers, so the sum depends neither on the edge order nor on where runs cross tile boundaries
+      const uint32_t live = __ballot_sync(0xffffffffu, dst_s >= 0);
+      long long s = 0;
 #pragma unroll
-    for (int le = 0; le < 32; ++le) {
+      for (int le = 0; le < 32; ++le) {
+        float v = 0.f;
 #pragma unroll
-      for (int c = 0; c < NCOPY; ++c) s += col[(c * 64 + le) * LD];
-      if (le == 31 || ((head_mask >> (le + 1)) & 1)) {          // warp-uniform: last edge of a run
-        const int dst = __shfl_sync(0xffffffffu, dst_s, le);
-        if constexpr (DFULL == DOUT) {
-          if (dst >= 0 && act) red_add(p.sum + (long long)dst * p.d_out + out_off + i, s);
-        } else {
-          const int w = i / DOUT;
-          if (dst >= 0 && act) red_add(p.sum + (long long)dst * p.d_out + out_off + w * DFULL + K0 + (i - w * DOUT), s);
+        for (int c = 0; c < NCOPY; ++c) v += col[(c * 64 + le) * LD];
+        if (act && ((live >> le) & 1)) s += to_fixed(v, p.err);
+        if (le == 31 || ((head_mask >> (le + 1)) & 1)) {        // warp-uniform: last edge of a run
+          const int dst = __shfl_sync(0xffffffffu, dst_s, le);
+          if constexpr (DFULL == DOUT) {
+            if (dst >= 0 && act) red_add_u64(p.sum_fx + (long long)dst * p.d_out + out_off + i, s);
+          } else {
+            const int w = i / DOUT;
+            if (dst >= 0 && act)
+              red_add_u64(p.sum_fx + (long long)dst * p.d_out + out_off + w * DFULL + K0 + (i - w * DOUT), s);
+          }
+          s = 0;
         }
-        s = 0.f;
+      }
+    } else {
+      float s = 0.f;
+#pragma unroll
+      for (int le = 0; le < 32; ++le) {
+#pragma unroll
+        for (int c = 0; c < NCOPY; ++c) s += col[(c * 64 + le) * LD];
+        if (le == 31 || ((head_mask >> (le + 1)) & 1)) {          // warp-uniform: last edge of a run
+          const int dst = __shfl_sync(0xffffffffu, dst_s, le);
+          if constexpr (DFULL == DOUT) {
+            if (dst >= 0 && act) red_add(p.sum + (long long)dst * p.d_out + out_off + i, s);
+          } else {
+            const int w = i / DOUT;
+            if (dst >= 0 && act) red_add(p.sum + (long long)dst * p.d_out + out_off + w * DFULL + K0 + (i - w * DOUT), s);
+          }
+          s = 0.f;
+        }
       }
     }
   }
@@ -574,7 +614,7 @@ template <bool SO> constexpr size_t smem_bytes() {
 // d_out <= 5, kinds 0-7, <= 32 paths); a (10, 5) tile (kind 6) would need 100 partial sums beside the 96 accumulator
 // registers, so it contracts its block in two slices, components 0-2 then 3-4, from the same accumulator tile and scatters
 // each slice at the end of the tile (not of the output irrep): 60 and 40 partial sums, the budget of kind 1.
-template <bool SO>
+template <bool SO, bool FIXED>
 __device__ __forceinline__ void fused_conv_body(const FusedParams& p) {
   constexpr int NST = SO ? SO_STAGES : STAGES;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -770,24 +810,24 @@ __device__ __forceinline__ void fused_conv_body(const FusedParams& p) {
 #pragma unroll
             for (int i = 0; i < NACC_MAX; ++i) acc[i] = 0.f;
             contract<10, 3, 16>(d, zcon, nch, q, acc);
-            flush<10, 3, 5, 0>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar);
+            flush<10, 3, 5, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar);
 #pragma unroll
             for (int i = 0; i < NACC_MAX; ++i) acc[i] = 0.f;
             contract<10, 2, 16, 3>(d, zcon, nch, q, acc, zconb);
-            flush<10, 2, 5, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar);
+            flush<10, 2, 5, 3, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar);
             break;
           case 7: contract<4, 5, 16>(d, zcon, nch, q, acc, zconb); break;
           default: __trap();
         }
         if ((flags & 2) && kind != 6) {
           switch (kind) {
-            case 0: flush<48, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 1: flush<10, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 2: flush<16, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 3: flush<4, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 4: flush<10, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 5: flush<4, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 7: flush<4, 5>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 0: flush<48, 1, 1, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 1: flush<10, 3, 3, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 2: flush<16, 1, 1, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 3: flush<4, 3, 3, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 4: flush<10, 1, 1, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 5: flush<4, 1, 1, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 7: flush<4, 5, 5, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
             default: __trap();
           }
         }
@@ -803,12 +843,12 @@ __device__ __forceinline__ void fused_conv_body(const FusedParams& p) {
         }
         if (flags & 2) {
           switch (kind) {
-            case 0: flush<48, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 1: flush<10, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 2: flush<16, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 3: flush<4, 3>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 4: flush<10, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
-            case 5: flush<4, 1>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 0: flush<48, 1, 1, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 1: flush<10, 3, 3, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 2: flush<16, 1, 1, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 3: flush<4, 3, 3, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 4: flush<10, 1, 1, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
+            case 5: flush<4, 1, 1, 0, FIXED>(p, acc, buf, r0, q, w4, lane, dst_s, head_mask, out_off, bar); break;
             default: __trap();
           }
         }
@@ -836,13 +876,16 @@ __device__ __forceinline__ void fused_conv_body(const FusedParams& p) {
   }
 }
 
-__global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParams p) { fused_conv_body<false>(p); }
-__global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel_so(const FusedParams p) { fused_conv_body<true>(p); }
+__global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel(const FusedParams p) { fused_conv_body<false, false>(p); }
+__global__ void __launch_bounds__(THREADS, 1) fused_conv_kernel_so(const FusedParams p) { fused_conv_body<true, false>(p); }
+// deterministic instantiations: the scatter adds 64-bit fixed-point values (ddb200_fused_conv_fixed / _so_fixed)
+__global__ void __launch_bounds__(THREADS, 1) fused_conv_fixed_kernel(const FusedParams p) { fused_conv_body<false, true>(p); }
+__global__ void __launch_bounds__(THREADS, 1) fused_conv_fixed_kernel_so(const FusedParams p) { fused_conv_body<true, true>(p); }
 
 // per-device state: debug counters and the one-time opt-in to > 48 KB of dynamic shared memory
 constexpr int MAX_DEVICES = 64;
 struct DeviceState {
-  bool attr_done = false, attr_done_so = false;
+  bool attr_done[2][2] = {};                      // [SO][FIXED]
   bool dbg_init = false;
   unsigned long long* dbg = nullptr;
 };
@@ -881,9 +924,11 @@ extern "C" int ddb200_fused_debug_read(uint64_t* out) {
 
 namespace {
 
-template <bool SO>
-int fused_conv_launch(const ddb200_fused_args* a, void* stream) {
-  if (!a || !a->edge_attr || !a->w1_images || !a->w2_images || !a->tiles || !a->mtab || !a->x || !a->edge_vec || !a->sum ||
+template <bool SO, bool FIXED>
+int fused_conv_launch(const ddb200_fused_args* a, long long* sum_fx, int* err, void* stream) {
+  if (FIXED && (!sum_fx || !err)) return DDB200_EINVAL;
+  if (!a || !a->edge_attr || !a->w1_images || !a->w2_images || !a->tiles || !a->mtab || !a->x || !a->edge_vec ||
+      (!FIXED && !a->sum) ||
       !a->tgt || !a->src || a->n_edges < 0 || a->ne <= 0 || a->ns < 0 || a->hidden <= 0 || a->n_tiles <= 0 || a->d_out <= 0)
     return DDB200_EINVAL;
   if (a->ns > 0 && (!a->node || a->ld_node < a->ns)) return DDB200_EINVAL;
@@ -916,6 +961,7 @@ int fused_conv_launch(const ddb200_fused_args* a, void* stream) {
   p.x = a->x; p.ld_x = a->ld_x; p.x_vec2 = (a->x_pairs_ok && (a->ld_x & 1) == 0 && (reinterpret_cast<uintptr_t>(a->x) & 7) == 0) ? 1 : 0;
   p.vec = a->edge_vec; p.ew = a->edge_weight; p.lmax = a->sh_lmax; p.sum = a->sum; p.d_out = a->d_out; p.cnt = a->cnt;
   p.n_edges = a->n_edges; p.n_edges_dev = a->n_edges_dev;
+  p.sum_fx = sum_fx; p.err = err;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= MAX_DEVICES) return DDB200_EINVAL;
@@ -924,8 +970,8 @@ int fused_conv_launch(const ddb200_fused_args* a, void* stream) {
   const long long n_mtiles = (a->n_edges + CTA_EDGES - 1) / CTA_EDGES;
   const size_t smem = smem_bytes<SO>();
   if (smem > 227 * 1024) return DDB200_ESMEM;
-  auto kernel = SO ? fused_conv_kernel_so : fused_conv_kernel;
-  bool& attr_done = SO ? g_dev[dev].attr_done_so : g_dev[dev].attr_done;
+  auto kernel = FIXED ? (SO ? fused_conv_fixed_kernel_so : fused_conv_fixed_kernel) : (SO ? fused_conv_kernel_so : fused_conv_kernel);
+  bool& attr_done = g_dev[dev].attr_done[SO][FIXED];
   if (!attr_done) {                 // the opt-in is a per-device, per-kernel attribute
     const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
@@ -938,8 +984,20 @@ int fused_conv_launch(const ddb200_fused_args* a, void* stream) {
 
 }  // namespace
 
-extern "C" int ddb200_fused_conv(const ddb200_fused_args* a, void* stream) { return fused_conv_launch<false>(a, stream); }
+extern "C" int ddb200_fused_conv(const ddb200_fused_args* a, void* stream) {
+  return fused_conv_launch<false, false>(a, nullptr, nullptr, stream);
+}
 
 // The second-order instantiation: plans with a 5-component input or output block (fused.py:FusedPlan.second_order); the
 // Clebsch-Gordan tables are [n_paths][5][5][5] padded to 128 floats.
-extern "C" int ddb200_fused_conv_so(const ddb200_fused_args* a, void* stream) { return fused_conv_launch<true>(a, stream); }
+extern "C" int ddb200_fused_conv_so(const ddb200_fused_args* a, void* stream) {
+  return fused_conv_launch<true, false>(a, nullptr, nullptr, stream);
+}
+
+// Deterministic instantiations (include/diffdock_b200.h): a->sum is ignored; the sums go to sum_fx in units of 2^-32.
+extern "C" int ddb200_fused_conv_fixed(const ddb200_fused_args* a, int64_t* sum_fx, int32_t* err, void* stream) {
+  return fused_conv_launch<false, true>(a, reinterpret_cast<long long*>(sum_fx), err, stream);
+}
+extern "C" int ddb200_fused_conv_so_fixed(const ddb200_fused_args* a, int64_t* sum_fx, int32_t* err, void* stream) {
+  return fused_conv_launch<true, true>(a, reinterpret_cast<long long*>(sum_fx), err, stream);
+}

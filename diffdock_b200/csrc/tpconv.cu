@@ -19,6 +19,7 @@
 #include <string.h>
 
 #include "../../include/diffdock_b200.h"
+#include "../../include/diffdock_b200_fixed.h"
 
 namespace {
 
@@ -37,6 +38,7 @@ struct KParams {
   const float* w; long long w_stride;
   long long n_edges;
   float* sum; float* cnt;
+  long long* sum_fx; int* err;    // deterministic kernel: int64 accumulator in units of 2^-32, sticky error word
   const int* iblob; const float* fblob;
   int n_ints, n_terms;
   int stages, warps;
@@ -80,6 +82,20 @@ __device__ __forceinline__ uint64_t policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
   return p;
+}
+
+// ---- deterministic scatter: every edge's output values are converted to 64-bit fixed point (v * 2^32, rounded to nearest)
+// and a row is summed as integers, so that its sum does not depend on the order of its edges or on how they are split
+// over warps, launches or kernels.  |v| >= 2^31 and non-finite values saturate and set the sticky error word (bit 0).
+constexpr int MAX_FX = 8;         // output values per lane: D_out <= 256
+__device__ __forceinline__ long long to_fixed(float v, int* err) {
+  const float s = v * 0x1p32f;
+  if (fabsf(s) < 0x1p63f) return __float2ll_rn(s);
+  atomicOr(err, 1);
+  return v > 0.f ? 0x7fffffffffffffffLL : (v < 0.f ? -0x7fffffffffffffffLL : 0LL);
+}
+__device__ __forceinline__ void red_add_u64(long long* addr, long long v) {
+  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(addr), "l"((unsigned long long)v) : "memory");
 }
 
 // ---- weight-tile contraction: acc[v*DOUT+k] += W[u, c*VEC+v] * z[u, k] over this lane's rows of the tile -----------
@@ -131,7 +147,8 @@ __device__ __noinline__ void run_rows_generic(const float* __restrict__ wp, cons
   }
 }
 
-__global__ void __launch_bounds__(512, 1) tpconv_accumulate_kernel(const KParams p) {
+template <bool FIXED>
+__device__ __forceinline__ void tpconv_accumulate_body(const KParams& p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 
@@ -230,18 +247,32 @@ __global__ void __launch_bounds__(512, 1) tpconv_accumulate_kernel(const KParams
   uint32_t c_par = 0;
   const int nxr = (D_in + WARP - 1) / WARP;
 
+  long long fx[FIXED ? MAX_FX : 1];          // FIXED: this lane's output values o = lane + 32 j of the current row
+#pragma unroll
+  for (int j = 0; j < (FIXED ? MAX_FX : 1); ++j) fx[j] = 0;
   auto flush_row = [&](int row, int row_edges) {
     __syncwarp();
-    float* srow = p.sum + (long long)row * D_out;
-    for (int o = lane; o < D_out; o += WARP) {
-      const int* om = outmap + 3 * o;
-      float v = 0.f;
-      for (int r = 0; r < om[2]; ++r) v += racc[om[0] + r * om[1]];
-      atomicAdd(srow + o, v);
+    if constexpr (FIXED) {
+      long long* srow = p.sum_fx + (long long)row * D_out;
+#pragma unroll
+      for (int j = 0; j < MAX_FX; ++j) {
+        if (lane + WARP * j < D_out) red_add_u64(srow + lane + WARP * j, fx[j]);
+        fx[j] = 0;
+      }
+    } else {
+      float* srow = p.sum + (long long)row * D_out;
+      for (int o = lane; o < D_out; o += WARP) {
+        const int* om = outmap + 3 * o;
+        float v = 0.f;
+        for (int r = 0; r < om[2]; ++r) v += racc[om[0] + r * om[1]];
+        atomicAdd(srow + o, v);
+      }
     }
     if (p.cnt && lane == 0) atomicAdd(p.cnt + row, (float)row_edges);
-    __syncwarp();
-    for (int j = lane; j < n_acc * WARP; j += WARP) racc[j] = 0.f;
+    if constexpr (!FIXED) {       // FIXED: the accumulators were cleared after the row's last edge
+      __syncwarp();
+      for (int j = lane; j < n_acc * WARP; j += WARP) racc[j] = 0.f;
+    }
   };
 
   for (long long unit = gw; unit < n_units; unit += TW) {
@@ -441,10 +472,30 @@ __global__ void __launch_bounds__(512, 1) tpconv_accumulate_kernel(const KParams
           }
         }
       }
+      if constexpr (FIXED) {      // this edge's output values alone (racc was clear before it), converted and summed
+        __syncwarp();
+#pragma unroll
+        for (int j = 0; j < MAX_FX; ++j) {
+          const int o = lane + WARP * j;
+          if (o < D_out) {
+            const int* om = outmap + 3 * o;
+            float v = 0.f;
+            for (int r = 0; r < om[2]; ++r) v += racc[om[0] + r * om[1]];
+            fx[j] += to_fixed(v, p.err);
+          }
+        }
+        __syncwarp();
+        for (int j = lane; j < n_acc * WARP; j += WARP) racc[j] = 0.f;
+        __syncwarp();
+      }
     }
     if (cur_row >= 0) flush_row(cur_row, row_edges);   // last row of this run
   }
 }
+
+__global__ void __launch_bounds__(512, 1) tpconv_accumulate_kernel(const KParams p) { tpconv_accumulate_body<false>(p); }
+// deterministic instantiation (ddb200_tpconv_accumulate_fixed)
+__global__ void __launch_bounds__(512, 1) tpconv_accumulate_fixed_kernel(const KParams p) { tpconv_accumulate_body<true>(p); }
 
 __global__ void tpconv_finalize_kernel(const float* __restrict__ sum, const float* __restrict__ cnt, long long n_rows,
                                        int d_out, int mean, const float* __restrict__ bn_scale,
@@ -457,6 +508,24 @@ __global__ void tpconv_finalize_kernel(const float* __restrict__ sum, const floa
     const int c = (int)(i - n * d_out);
     float v = sum[i];
     if (mean) v = v / fmaxf(cnt[n], 1.1920928955078125e-07f);   // torch.finfo(float32).eps, tensor_layers.py:228
+    if (bn_scale) v = fmaf(v, bn_scale[c], bn_shift[c]);
+    if (residual && c < res_dim) v += residual[n * res_stride + c];
+    out[i] = v;
+  }
+}
+
+// the epilogue over fixed-point sums: the mean is formed in double from the exact integer sum and rounded once to fp32
+__global__ void tpconv_finalize_fixed_kernel(const long long* __restrict__ sum, const float* __restrict__ cnt,
+                                             long long n_rows, int d_out, int mean, const float* __restrict__ bn_scale,
+                                             const float* __restrict__ bn_shift, const float* __restrict__ residual,
+                                             long long res_stride, int res_dim, float* __restrict__ out) {
+  const long long total = n_rows * d_out;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const long long n = i / d_out;
+    const int c = (int)(i - n * d_out);
+    const double s = (double)sum[i] * 0x1p-32;
+    float v = mean ? (float)(s / (double)fmaxf(cnt[n], 1.1920928955078125e-07f)) : (float)s;
     if (bn_scale) v = fmaf(v, bn_scale[c], bn_shift[c]);
     if (residual && c < res_dim) v += residual[n * res_stride + c];
     out[i] = v;
@@ -526,6 +595,8 @@ int ddb200_tp_table_create(const int32_t* ib, int n_ints, const float* fb, int n
   if (e == cudaSuccess) e = cudaMemcpy(t->d_fblob, fb, sizeof(float) * n_floats, cudaMemcpyHostToDevice);
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(tpconv_accumulate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(tpconv_accumulate_fixed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   if (e != cudaSuccess) { ddb200_tp_table_destroy(t); return (int)e; }
   *out = t;
   return 0;
@@ -553,16 +624,22 @@ int ddb200_tp_table_info(const ddb200_tp_table* t, int what) {
   }
 }
 
-int ddb200_tpconv_accumulate(const ddb200_tp_table* t, const float* x, int64_t x_stride, const int32_t* edge_src,
-                             const int32_t* edge_dst, const float* geo, const float* edge_weight, const float* w,
-                             int64_t w_stride, int64_t n_edges, float* sum, float* cnt, void* stream) {
-  if (!t || !x || !edge_src || !edge_dst || !geo || !w || !sum || n_edges < 0) return DDB200_EINVAL;
+}  // extern "C"
+
+static int tpconv_accumulate_launch(const ddb200_tp_table* t, const float* x, int64_t x_stride, const int32_t* edge_src,
+                                    const int32_t* edge_dst, const float* geo, const float* edge_weight, const float* w,
+                                    int64_t w_stride, int64_t n_edges, float* sum, long long* sum_fx, int* err, float* cnt,
+                                    void* stream) {
+  const bool fixed = sum_fx != nullptr;
+  if (!t || !x || !edge_src || !edge_dst || !geo || !w || !(fixed ? (err != nullptr) : (sum != nullptr)) || n_edges < 0)
+    return DDB200_EINVAL;
+  if (fixed && t->hdr[8] > WARP * MAX_FX) return DDB200_EINVAL;
   if (n_edges == 0) return 0;
   if ((reinterpret_cast<uintptr_t>(w) & 15) || (w_stride & 3) || w_stride < t->hdr[13] || x_stride < t->hdr[6])
     return DDB200_EINVAL;
   KParams p;
   p.x = x; p.x_stride = x_stride; p.esrc = edge_src; p.edst = edge_dst; p.geo = geo; p.ew = edge_weight;
-  p.w = w; p.w_stride = w_stride; p.n_edges = n_edges; p.sum = sum; p.cnt = cnt;
+  p.w = w; p.w_stride = w_stride; p.n_edges = n_edges; p.sum = sum; p.cnt = cnt; p.sum_fx = sum_fx; p.err = err;
   p.iblob = t->d_iblob; p.fblob = t->d_fblob; p.n_ints = t->n_ints; p.n_terms = t->n_terms;
   p.stages = t->stages; p.warps = t->warps; p.warp_floats = t->warp_floats; p.stage_floats = t->hdr[14];
   p.warp_base_off = t->warp_base_off;
@@ -572,8 +649,29 @@ int ddb200_tpconv_accumulate(const ddb200_tp_table* t, const float* x, int64_t x
   const long long units = (n_edges + ERUN - 1) / ERUN;
   long long ctas = (units + t->warps - 1) / t->warps;
   if (ctas > sms) ctas = sms;   // persistent: one CTA per SM, warps stride over the edge runs
-  tpconv_accumulate_kernel<<<(unsigned)ctas, t->warps * WARP, t->smem_bytes, (cudaStream_t)stream>>>(p);
+  if (fixed)
+    tpconv_accumulate_fixed_kernel<<<(unsigned)ctas, t->warps * WARP, t->smem_bytes, (cudaStream_t)stream>>>(p);
+  else
+    tpconv_accumulate_kernel<<<(unsigned)ctas, t->warps * WARP, t->smem_bytes, (cudaStream_t)stream>>>(p);
   return (int)cudaGetLastError();
+}
+
+extern "C" {
+
+int ddb200_tpconv_accumulate(const ddb200_tp_table* t, const float* x, int64_t x_stride, const int32_t* edge_src,
+                             const int32_t* edge_dst, const float* geo, const float* edge_weight, const float* w,
+                             int64_t w_stride, int64_t n_edges, float* sum, float* cnt, void* stream) {
+  return tpconv_accumulate_launch(t, x, x_stride, edge_src, edge_dst, geo, edge_weight, w, w_stride, n_edges, sum, nullptr,
+                                  nullptr, cnt, stream);
+}
+
+int ddb200_tpconv_accumulate_fixed(const ddb200_tp_table* t, const float* x, int64_t x_stride, const int32_t* edge_src,
+                                   const int32_t* edge_dst, const float* geo, const float* edge_weight, const float* w,
+                                   int64_t w_stride, int64_t n_edges, int64_t* sum, float* cnt, int32_t* err,
+                                   void* stream) {
+  if (!sum) return DDB200_EINVAL;
+  return tpconv_accumulate_launch(t, x, x_stride, edge_src, edge_dst, geo, edge_weight, w, w_stride, n_edges, nullptr,
+                                  reinterpret_cast<long long*>(sum), err, cnt, stream);
 }
 
 int ddb200_tpconv_finalize(const float* sum, const float* cnt, int64_t n_rows, int d_out, int mean,
@@ -587,6 +685,21 @@ int ddb200_tpconv_finalize(const float* sum, const float* cnt, int64_t n_rows, i
   if (blocks > 132 * 16) blocks = 132 * 16;
   tpconv_finalize_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(sum, cnt, n_rows, d_out, mean, bn_scale,
                                                                             bn_shift, residual, res_stride, res_dim, out);
+  return (int)cudaGetLastError();
+}
+
+int ddb200_tpconv_finalize_fixed(const int64_t* sum, const float* cnt, int64_t n_rows, int d_out, int mean,
+                                 const float* bn_scale, const float* bn_shift, const float* residual, int64_t res_stride,
+                                 int res_dim, float* out, void* stream) {
+  if (!sum || !out || n_rows < 0 || d_out <= 0 || (mean && !cnt) || ((bn_scale == nullptr) != (bn_shift == nullptr)))
+    return DDB200_EINVAL;
+  if (n_rows == 0) return 0;
+  const long long total = n_rows * (long long)d_out;
+  long long blocks = (total + 255) / 256;
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  tpconv_finalize_fixed_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const long long*>(sum), cnt, n_rows, d_out, mean, bn_scale, bn_shift, residual, res_stride, res_dim,
+      out);
   return (int)cudaGetLastError();
 }
 

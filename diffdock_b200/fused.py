@@ -41,7 +41,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .ops import PROFILE, _need_cuda, _ptr, _stream
+from .ops import PROFILE, _need_cuda, _ptr, _stream, fixed_error_word
 
 from .irreps import real_cg
 from .radial import BK, BN
@@ -223,7 +223,7 @@ def fused_conv(plan: FusedPlan, edge_attr, node, ns, tgt32, src32, x, edge_vec, 
         return
     t = plan.table
     assert edge_attr.dtype == torch.float32 and edge_attr.stride(1) == 1 and x.stride(1) == 1 and edge_vec.is_contiguous()
-    assert edge_vec.dtype == torch.float32 and x.dtype == torch.float32 and sum_buf.dtype == torch.float32
+    assert edge_vec.dtype == torch.float32 and x.dtype == torch.float32 and sum_buf.dtype in (torch.float32, torch.int64)
     assert tgt32.dtype == torch.int32 and src32.dtype == torch.int32 and tgt32.is_contiguous() and src32.is_contiguous()
     assert ne + 2 * ns == plan.k1 and x.shape[1] == t.d_in and sum_buf.shape[1] == t.d_out and sum_buf.is_contiguous()
     if edge_perm is None:
@@ -238,17 +238,24 @@ def fused_conv(plan: FusedPlan, edge_attr, node, ns, tgt32, src32, x, edge_vec, 
         assert ea_add_idx.dtype == torch.int32 and ea_add_idx.is_contiguous() and ea_add_idx.shape[0] >= E
     if n_edges_dev is not None:
         assert n_edges_dev.dtype == torch.int32 and n_edges_dev.is_cuda
+    fixed = sum_buf.dtype == torch.int64     # fixed-point accumulators (ops.new_accumulators under the deterministic flag)
     a = _Args(_p(edge_attr), edge_attr.stride(0), ne, _p(node) if ns else None, node.stride(0) if ns else 0, ns,
               _p(tgt32), _p(src32), _p(edge_perm), _p(ea_add), _p(ea_add_idx) if ea_add is not None else None,
               float(vec_sign), _p(plan.w1_images), plan.hidden, _p(plan.w2_images), _p(plan.tiles), plan.n_tiles,
               _p(plan.mtab), plan.n_paths, _p(x), x.stride(0), plan.x_pairs_ok, _p(edge_vec), _p(edge_weight),
-              t.sh_lmax, E, _p(n_edges_dev), _p(sum_buf), t.d_out, _p(cnt_buf), _p(plan.wh_images), plan.n_hidden)
+              t.sh_lmax, E, _p(n_edges_dev), None if fixed else _p(sum_buf), t.d_out, _p(cnt_buf), _p(plan.wh_images),
+              plan.n_hidden)
     prof = PROFILE.enabled
     if prof:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-    launch = _lib.lib().ddb200_fused_conv_so if plan.second_order else _lib.lib().ddb200_fused_conv
-    rc = launch(C.byref(a), _stream())
+    L = _lib.lib()
+    if fixed:
+        launch = L.ddb200_fused_conv_so_fixed if plan.second_order else L.ddb200_fused_conv_fixed
+        rc = launch(C.byref(a), _p(sum_buf), _p(fixed_error_word(sum_buf.device)), _stream())
+    else:
+        launch = L.ddb200_fused_conv_so if plan.second_order else L.ddb200_fused_conv
+        rc = launch(C.byref(a), _stream())
     if prof:
         e1.record()
         n_live = int(n_edges_dev.item()) if n_edges_dev is not None else E      # profiling replay only (host sync)
@@ -258,4 +265,4 @@ def fused_conv(plan: FusedPlan, edge_attr, node, ns, tgt32, src32, x, edge_vec, 
         PROFILE.fused_flops += ((n_live + 63) // 64) * plan.mma_flops_per_tile
         PROFILE.fused_alg_flops += n_live * plan.alg_flops_per_edge
     PROFILE.all_launches += 1
-    _lib.check(rc, 'ddb200_fused_conv')
+    _lib.check(rc, 'ddb200_fused_conv_fixed' if fixed else 'ddb200_fused_conv')

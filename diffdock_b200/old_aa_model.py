@@ -349,8 +349,7 @@ class AAOldModel(nn.Module):
                                                (5, 'ar', o_a, N, slice(nr_u, n_u), map_a)):
             tgt, src, perm = local[key]
             s0, n0 = convs[k].accumulate_group(x0, (tgt, src, *g[key][2:5], dict(edge_perm=perm)), 0, n_u, self.ns)
-            s = torch.zeros((hi, D), device=x.device)
-            n = torch.zeros((hi,), device=x.device)
+            s, n = ops.new_accumulators(hi, D, x.device)
             s[lo:] = s0[part][node_map]
             n[lo:] = n0[part][node_map]
             acc[k] = (s, n)

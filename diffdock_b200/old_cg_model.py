@@ -290,8 +290,7 @@ class CGOldModel(nn.Module):
             last = l == L - 1
             n_out = n_lig if last else x.shape[0]
             D = self.lig_conv_layers[l].out_size
-            intra = (torch.zeros((n_out, D), device=x.device), torch.zeros((n_out,), device=x.device))
-            inter = (torch.zeros((n_out, D), device=x.device), torch.zeros((n_out,), device=x.device))
+            intra, inter = ops.new_accumulators(n_out, D, x.device), ops.new_accumulators(n_out, D, x.device)
             self.lig_conv_layers[l].accumulate_group(x, g_ll, 0, n_out, ns, init=intra)
             self.rec_to_lig_conv_layers[l].accumulate_group(x, g_lr, 0, n_out, ns, init=inter)
             if not last:

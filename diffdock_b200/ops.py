@@ -1,6 +1,8 @@
 """Tensor-level wrappers over the C ABI (device pointers + current CUDA stream).  CUDA tensors only.
 
 What each wrapper stands in for in the reference (details per entry point in include/diffdock_b200.h):
+  deterministic / new_accumulators /    the convolutions' fixed-point scatter under torch.use_deterministic_algorithms(True)
+  check_fixed_error
   tpconv_accumulate / tpconv_finalize   gather + o3.spherical_harmonics + tensor product + torch_scatter.scatter + bincount and
                                         the mean / BatchNorm / residual epilogue, models/tensor_layers.py:139-144,204-229,327-332
   radius                                torch_cluster.radius / radius_graph, models/cg_model.py:477,543-548,630
@@ -56,6 +58,54 @@ class _Profile:
 PROFILE = _Profile()
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# Deterministic convolutions.  Under torch.use_deterministic_algorithms(True) the convolution accumulators are int64 sums
+# of 64-bit fixed-point values (2^-32 units, include/diffdock_b200.h: ddb200_tpconv_accumulate_fixed): integer addition is
+# associative, so a forward gives the same bits whatever order the scatter reductions land in.  The flag is read where the
+# accumulators are allocated (``new_accumulators``); every launch that takes an accumulator follows its dtype.
+FIXED_SCALE = 2.0 ** 32
+FIXED_LIMIT = 2.0 ** 31          # |value| of one edge (and of a sum) the fixed-point accumulators hold
+
+
+def deterministic():
+    """True when the convolutions use the fixed-point scatter: ``torch.are_deterministic_algorithms_enabled()``."""
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def new_accumulators(n_rows, d_out, device):
+    """Zeroed convolution accumulators ``(sum [n_rows, d_out], cnt [n_rows] fp32)``; ``sum`` is int64 fixed point when
+    ``deterministic()``, else fp32."""
+    dt = torch.int64 if deterministic() else torch.float32
+    return (torch.zeros((n_rows, d_out), dtype=dt, device=device), torch.zeros((n_rows,), dtype=torch.float32, device=device))
+
+
+_FIXED_ERR = {}
+
+
+def fixed_error_word(device):
+    """The device's sticky int32 error word of the fixed-point scatter (set when a value leaves the range).  Created on
+    first use, which must not be inside a CUDA-graph capture (``GraphedSteps`` creates it before capturing)."""
+    dev = torch.device(device)
+    key = dev.index if dev.index is not None else torch.cuda.current_device()
+    w = _FIXED_ERR.get(key)
+    if w is None:
+        w = _FIXED_ERR[key] = torch.zeros(1, dtype=torch.int32, device=torch.device('cuda', key))
+    return w
+
+
+def check_fixed_error(device=None):
+    """Raise RuntimeError if a fixed-point scatter on ``device`` (None: every device used) saturated since the last check,
+    and clear the word.  One device-to-host read per device; nothing to read when no fixed-point launch ran."""
+    keys = list(_FIXED_ERR) if device is None else [torch.device(device).index if torch.device(device).index is not None
+                                                    else torch.cuda.current_device()]
+    for k in keys:
+        w = _FIXED_ERR.get(k)
+        if w is not None and int(w.item()):
+            w.zero_()
+            raise RuntimeError(f"deterministic convolution on cuda:{k}: a message value or sum left the fixed-point range "
+                               f"|x| < 2^31 (torch.use_deterministic_algorithms(True))")
+
+
 class TpHandle:
     """Device-resident tensor-product table (ddb200_tp_table)."""
 
@@ -94,6 +144,7 @@ def tpconv_accumulate(h: TpHandle, x, edge_src, edge_dst, geo, w, sum_buf, cnt_b
         return
     t = h.table
     assert x.dtype == torch.float32 and w.dtype == torch.float32 and geo.dtype == torch.float32
+    assert sum_buf.dtype in (torch.float32, torch.int64)
     assert edge_src.dtype == torch.int32 and edge_dst.dtype == torch.int32
     assert x.stride(1) == 1 and w.stride(1) == 1 and geo.is_contiguous() and sum_buf.is_contiguous()
     assert edge_src.is_contiguous() and edge_dst.is_contiguous()
@@ -106,9 +157,14 @@ def tpconv_accumulate(h: TpHandle, x, edge_src, edge_dst, geo, w, sum_buf, cnt_b
     if prof:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-    rc = _lib.lib().ddb200_tpconv_accumulate(h._h, _ptr(x), x.stride(0), _ptr(edge_src), _ptr(edge_dst), _ptr(geo),
-                                             _ptr(edge_weight), _ptr(w), w.stride(0), E, _ptr(sum_buf), _ptr(cnt_buf),
-                                             _stream())
+    if sum_buf.dtype == torch.int64:        # fixed-point accumulators (new_accumulators under the deterministic flag)
+        rc = _lib.lib().ddb200_tpconv_accumulate_fixed(h._h, _ptr(x), x.stride(0), _ptr(edge_src), _ptr(edge_dst), _ptr(geo),
+                                                       _ptr(edge_weight), _ptr(w), w.stride(0), E, _ptr(sum_buf),
+                                                       _ptr(cnt_buf), _ptr(fixed_error_word(sum_buf.device)), _stream())
+    else:
+        rc = _lib.lib().ddb200_tpconv_accumulate(h._h, _ptr(x), x.stride(0), _ptr(edge_src), _ptr(edge_dst), _ptr(geo),
+                                                 _ptr(edge_weight), _ptr(w), w.stride(0), E, _ptr(sum_buf), _ptr(cnt_buf),
+                                                 _stream())
     if prof:
         e1.record()
         PROFILE.pairs.append((e0, e1))
@@ -116,21 +172,24 @@ def tpconv_accumulate(h: TpHandle, x, edge_src, edge_dst, geo, w, sum_buf, cnt_b
         if count_node_bytes:   # node tensors are compulsory traffic once per (layer, edge set), not per edge block
             PROFILE.bytes += 4 * (sum_buf.shape[0] + 1) + 4 * x.shape[0] * t.d_in + 4 * sum_buf.shape[0] * t.d_out
     PROFILE.all_launches += 1
-    _lib.check(rc, 'ddb200_tpconv_accumulate')
+    _lib.check(rc, 'ddb200_tpconv_accumulate_fixed' if sum_buf.dtype == torch.int64 else 'ddb200_tpconv_accumulate')
 
 
 def tpconv_finalize(sum_buf, cnt_buf, mean, bn_scale=None, bn_shift=None, residual=None, out=None):
+    """The epilogue into fp32 ``out``; int64 (fixed-point) ``sum_buf`` takes ddb200_tpconv_finalize_fixed."""
     _need_cuda(sum_buf)
     n, d = sum_buf.shape
+    fixed = sum_buf.dtype == torch.int64
     if out is None:
-        out = torch.empty_like(sum_buf)
+        out = torch.empty(sum_buf.shape, dtype=torch.float32, device=sum_buf.device)
     res_stride = residual.stride(0) if residual is not None else 0
     res_dim = residual.shape[1] if residual is not None else 0
     if residual is not None:
         assert residual.stride(1) == 1 and residual.shape[0] == n and res_dim <= d
-    rc = _lib.lib().ddb200_tpconv_finalize(_ptr(sum_buf), _ptr(cnt_buf), n, d, 1 if mean else 0, _ptr(bn_scale),
-                                           _ptr(bn_shift), _ptr(residual), res_stride, res_dim, _ptr(out), _stream())
-    _lib.check(rc, 'ddb200_tpconv_finalize')
+    fin = _lib.lib().ddb200_tpconv_finalize_fixed if fixed else _lib.lib().ddb200_tpconv_finalize
+    rc = fin(_ptr(sum_buf), _ptr(cnt_buf), n, d, 1 if mean else 0, _ptr(bn_scale), _ptr(bn_shift), _ptr(residual),
+             res_stride, res_dim, _ptr(out), _stream())
+    _lib.check(rc, 'ddb200_tpconv_finalize_fixed' if fixed else 'ddb200_tpconv_finalize')
     PROFILE.all_launches += 1
     return out
 

@@ -311,7 +311,9 @@ class GraphedSteps:
             model._static(g)
         sig = (b, n_lig, n_rec, int(g['ligand', 'ligand'].edge_index.shape[1]), int(g['receptor', 'receptor'].edge_index.shape[1]),
                int(g._pose_layout[1].shape[0]) if packed else int(bond_u.shape[0]) if bond_u is not None else 0, draw_noise,
-               philox is not None, crop_rows is not None, frames is not None)
+               philox is not None, crop_rows is not None, frames is not None, ops.deterministic())
+        if ops.deterministic():
+            ops.fixed_error_word(device)         # the fixed-point scatter's error word exists before the capture
         seen = getattr(model, '_graph_warmed_shapes', None)
         if seen is None:
             seen = set()
@@ -626,6 +628,8 @@ def sampling(data_list, model, inference_steps, tr_schedule, rot_schedule, tor_s
             _add_frames(visualization_list, data_list, b0, frames.view(inference_steps, b, n, 3).cpu())
     if confidence_model is not None:
         confidence = torch.nan_to_num(torch.cat(confidence, dim=0), nan=-1000)
+    if ops.deterministic():
+        ops.check_fixed_error(device)
     return data_list, confidence
 
 
@@ -758,4 +762,6 @@ def sample_packed(complexes, model, inference_steps, tr_schedule, rot_schedule, 
                                                    finals[k], len(complexes[k]), device), nan=-1000) for k in range(K)]
     if errs and int(torch.stack(errs).max()):
         raise RuntimeError("ddb200_pose_update_packed met a pose outside the declared layout")
+    if ops.deterministic():
+        ops.check_fixed_error(device)
     return [(complexes[k], confidence[k]) for k in range(K)]

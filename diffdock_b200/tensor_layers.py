@@ -377,9 +377,8 @@ class TensorProductConvLayer(nn.Module):
         if init is not None:
             sum_buf, cnt_buf = init
             assert tuple(sum_buf.shape) == (n_out, self.out_size) and sum_buf.is_contiguous() and cnt_buf.shape[0] == n_out
-        else:
-            sum_buf = torch.zeros((n_out, self.out_size), dtype=torch.float32, device=x.device)
-            cnt_buf = torch.zeros((n_out,), dtype=torch.float32, device=x.device)
+        else:       # int64 fixed point under torch.use_deterministic_algorithms(True) (ops.new_accumulators)
+            sum_buf, cnt_buf = ops.new_accumulators(n_out, self.out_size, x.device)
         blk = None
         for item, fc in zip(prepared, fcs):
             if item is None:
