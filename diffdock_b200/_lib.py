@@ -56,6 +56,11 @@ FIXED_SIGNATURES = {
     'ddb200_fused_conv_so_fixed': (_int, [_vp, _vp, _vp, _vp]),
 }
 
+# the pose metrics of evaluation; mirrors include/diffdock_b200_metrics.h one to one
+METRICS_SIGNATURES = {
+    'ddb200_pose_metrics': (_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+}
+
 
 def lib():
     global _lib
@@ -65,7 +70,7 @@ def lib():
                 f"{LIB_PATH} not found: build the CUDA extension first (python -c 'import __graft_entry__ as g; "
                 f"g.build()').  diffdock_b200 has no CPU fallback.")
         _lib = C.CDLL(LIB_PATH)
-        for name, (res, args) in (SIGNATURES | FIXED_SIGNATURES).items():
+        for name, (res, args) in (SIGNATURES | FIXED_SIGNATURES | METRICS_SIGNATURES).items():
             fn = getattr(_lib, name)
             fn.restype, fn.argtypes = res, args
     return _lib
